@@ -1,4 +1,4 @@
-/* libw2b — C ABI of the B200-native Word2Bits training path.
+/* libw2b — C ABI of the H100-native Word2Bits training path.
  *
  * The reference (agnusmaximus/Word2Bits, src/word2bits.cpp) has no FFI: it is one
  * executable whose hot path is `void *TrainModelThread(void *id)` (:363-516) reading and
@@ -109,7 +109,7 @@ typedef struct {
                           1 = register kernel (one CTA per shard; also serves strict mode and D > 1024) */
   int32_t slots;       /* warp kernel: shared-memory row slots per warp (0 = as many as fit, at most 16) */
   int32_t prefetch;    /* warp kernel: 0 = the positions of a shard strictly one after another, like a reference
-                          thread (default; measured free on B200); 1 = rows of position p+1 are fetched before p's
+                          thread (default); 1 = rows of position p+1 are fetched before p's
                           updates have landed (a context row shared by neighbours is read one update stale) */
   int32_t sync_mode;   /* multi-GPU exchange (w2b_sync): 0 = replicas are averaged (default); 1 = every rank's
                           updates since the last exchange are summed onto the common base (needs two more tables;
@@ -207,7 +207,7 @@ int w2b_quantize(w2b_ctx *ctx, const float *in, float *out, int64_t n, int bitle
 /* Analogy evaluator (SURVEY section 8(f).2), replaces src/compute-accuracy.c:63-189: same inputs
  * (word2vec-binary vector file, optional re-quantisation, vocabulary threshold, question stream),
  * same report text; all questions are scored on the GPU: one Q x V x D TF32 tensor-core contraction
- * (tcgen05 + TMA) as a filter with a proven error bound, then an fp32 re-score of the surviving candidates in the
+ * (wgmma + TMA) as a filter with a proven error bound, then an fp32 re-score of the surviving candidates in the
  * reference's operation order, so the arg-max (ties included) is the reference's.  questions_file NULL = stdin.  report may be NULL. */
 typedef struct {
   int64_t questions_total, questions_seen, correct;

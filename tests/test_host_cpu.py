@@ -11,7 +11,7 @@ import numpy as np
 import pytest
 
 from oracle import pyoracle as po
-from tests.util import zipf_corpus
+from tests.util import digest, reference_outputs, zipf_corpus
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "word2bits_b200", "libw2b.so")
@@ -91,17 +91,16 @@ def test_corpus_edge_cases(tmp_path):
             assert [o.shard_start(i, n) for i in range(n)] == list(zip(s.tolist(), f.tolist())), (name, n)
 
 
-@pytest.mark.skipif(not po.ref_available("strict"), reason="oracle/_ref not built")
 def test_corpus_matches_reference(tmp_path):
+    """Vocabulary, counts and sizes equal what the unmodified reference's LearnVocabFromTrainFile computed on the
+    same corpus (tests/golden/reference_outputs.json)."""
     import word2bits_b200 as w2b
     path = zipf_corpus(str(tmp_path / "c.txt"), 80000, 5000, seed=5)
-    ref = po.Ref("strict")
     for mc in (1, 5):
-        ref.configure(path, 8, 3, 4, 1, min_count=mc)
-        ref.learn_vocab()
+        want = reference_outputs("host_cpu")["corpus_seed5_mc%d" % mc]
         c = w2b.Corpus(path, mc)
-        assert c.words() == ref.words() and np.array_equal(c.counts, ref.counts())
-        assert (c.train_words, c.file_size) == (ref.train_words, ref.file_size)
+        assert digest(c.words()) == want["words"] and digest(c.counts) == want["counts"]
+        assert (c.vocab_size, c.train_words, c.file_size) == (want["V"], want["train_words"], want["file_size"])
 
 
 def test_vector_writer_matches_oracle(tmp_path):
@@ -131,12 +130,9 @@ def test_cli_messages_and_exit_codes(tmp_path):
     assert ours[0] == (1, "Starting training using file /nonexistent\nERROR: training data file not found!\n")
     assert ours[1] == (1, "Argument missing for -train\n")
     assert ours[2] == (0, "Starting training using file %s\nVocab size: 31\nWords in train file: 13533\n" % golden)
-    refbin = os.path.join(ROOT, "oracle", "_ref", "word2bits")
-    if os.path.exists(refbin):
-        theirs = [run(refbin, "-train", "/nonexistent", "-output", "x"), run(refbin, "-train"),
-                  run(refbin, "-train", golden, "-min-count", "1"),
-                  run(refbin, "-train", golden, "-min-count", "5", "-debug", "0")]
-        assert ours == theirs
+    # the reference's own binary, same four calls
+    theirs = [(rc, out.replace("{golden}", golden)) for rc, out in reference_outputs("host_cpu")["cli_messages"]]
+    assert ours == theirs
 
 
 def test_parallel_tokenizer_equals_sequential(tmp_path, monkeypatch):
@@ -294,6 +290,17 @@ def test_streaming_slice_gather(nthreads):
     assert lib.w2b_host_gather_slices(None, n, L, S, ptr(cursor), ptr(done), ptr(stage), ptr(xl), ptr(lim), ptr(eof), 1) != 0
 
 
+def fuzz_corpus(path, seed):
+    rng = np.random.default_rng(100 + seed)
+    alphabet = np.frombuffer(b"abcde" * 6 + b"  \t\n\n\r\x00\x01\xff\xc3\xa9", np.uint8)
+    body = alphabet[rng.integers(0, len(alphabet), 400_000)].tobytes()
+    long_words = b" " + b"x" * 4094 + b" " + b"y" * 4095 + b" " + b"z" * 4096 + b"q " + b"k" * 9000 + b"\n"
+    data = body[:150_000] + long_words + body[150_000:] + (b"" if seed == 0 else b" tail" if seed == 1 else b"\r")
+    with open(path, "wb") as f:
+        f.write(data)
+    return path
+
+
 @pytest.mark.parametrize("seed", [0, 1, 2])
 def test_tokenizer_fuzz_against_oracle(tmp_path, monkeypatch, seed):
     """Random bytes from a hostile alphabet (CR and NUL inside words, control characters, high bytes, runs of
@@ -301,13 +308,7 @@ def test_tokenizer_fuzz_against_oracle(tmp_path, monkeypatch, seed):
     hashed straight from the mapping) and the byte-by-byte slow path must reproduce the reference's reader for
     every thread count — words, counts, token stream and shard starts."""
     import word2bits_b200 as w2b
-    rng = np.random.default_rng(100 + seed)
-    alphabet = np.frombuffer(b"abcde" * 6 + b"  \t\n\n\r\x00\x01\xff\xc3\xa9", np.uint8)
-    body = alphabet[rng.integers(0, len(alphabet), 400_000)].tobytes()
-    long_words = b" " + b"x" * 4094 + b" " + b"y" * 4095 + b" " + b"z" * 4096 + b"q " + b"k" * 9000 + b"\n"
-    data = body[:150_000] + long_words + body[150_000:] + (b"" if seed == 0 else b" tail" if seed == 1 else b"\r")
-    p = tmp_path / "fuzz.txt"
-    p.write_bytes(data)
+    p = fuzz_corpus(str(tmp_path / "fuzz.txt"), seed)
     o = po.Corpus(str(p), 2)
     monkeypatch.setenv("W2B_TOKENIZER_MIN_CHUNK", "20000")
     for threads in ("1", "3", "16"):
@@ -319,12 +320,9 @@ def test_tokenizer_fuzz_against_oracle(tmp_path, monkeypatch, seed):
         for n in (1, 7, 64):
             s, f = c.shards(n)
             assert [o.shard_start(i, n) for i in range(n)] == list(zip(s.tolist(), f.tolist())), (threads, n)
-    if po.ref_available("strict"):
-        ref = po.Ref("strict")
-        ref.configure(str(p), 8, 3, 4, 1, min_count=2)
-        ref.learn_vocab()
-        assert c.words() == ref.words() and np.array_equal(c.counts, ref.counts())
-        assert c.train_words == ref.train_words
+    want = reference_outputs("host_cpu")["tokenizer_fuzz%d" % seed]  # the unmodified reference's reader
+    assert digest(c.words()) == want["words"] and digest(c.counts) == want["counts"]
+    assert c.train_words == want["train_words"]
 
 
 def test_text_writer_parallel_and_cached_formatting(tmp_path, monkeypatch):
@@ -362,6 +360,9 @@ def _vector_file(path, words, D, seed=0):
             f.write(w.encode() + b" " + rng.standard_normal(D).astype(np.float32).tobytes() + b"\n")
 
 
+EMPTY_REPORT_QUESTIONS = ": capital-common-countries\nathens greece baghdad iraq\nzzz yyy xxx www\n: family\nboy girl zzz sister\n"
+
+
 def test_evaluator_host_side_errors_and_empty_report(tmp_path):
     """w2b_compute_accuracy (SURVEY 8(f).2) before any GPU work: bad arguments and unreadable / hostile vector files
     are error codes, never crashes or exceptions across the C ABI; a question stream in which no question can be
@@ -372,7 +373,7 @@ def test_evaluator_host_side_errors_and_empty_report(tmp_path):
     acc = w2b._lib.Accuracy()
     buf = C.create_string_buffer(4096)
     qf = tmp_path / "q.txt"
-    qf.write_text(": capital-common-countries\nathens greece baghdad iraq\nzzz yyy xxx www\n: family\nboy girl zzz sister\n")
+    qf.write_text(EMPTY_REPORT_QUESTIONS)
     call = lambda vf: lib.w2b_compute_accuracy(vf, 0, 0, str(qf).encode(), 0, C.byref(acc), buf, len(buf))
     assert call(None) == EINVAL
     assert call(str(tmp_path / "missing.bin").encode()) == 3 and b"not found" in lib.w2b_last_error()
@@ -386,10 +387,7 @@ def test_evaluator_host_side_errors_and_empty_report(tmp_path):
     _vector_file(vf, ["athens", "greece", "baghdad", "boy", "girl", "sister"], 8)
     got, counters = w2b.compute_accuracy(vf, str(qf))
     assert counters["questions_total"] == 3 and counters["questions_seen"] == 0 and counters["gpu_ms"] == 0.0
-    refbin = os.path.join(ROOT, "oracle", "_ref", "compute_accuracy")
-    if os.path.exists(refbin):
-        want = subprocess.run([refbin, vf, "0", "0"], stdin=open(qf), capture_output=True, text=True).stdout
-        assert got == want
+    assert got == reference_outputs("host_cpu")["evaluator_empty_report"]  # src/compute-accuracy.c's report
 
 
 def test_corpus_above_the_reduce_vocab_threshold_is_refused(tmp_path, monkeypatch):
@@ -410,9 +408,8 @@ def test_corpus_above_the_reduce_vocab_threshold_is_refused(tmp_path, monkeypatc
 
 
 def test_default_geometry_is_the_measured_one():
-    """The numbers under profiles/ (round 2) were measured with these launch geometries of the production kernel: one
-    32-thread CTA per shard, `warps_per_sm` of them resident per SM.  Pinned so that a planner change cannot move the
-    benchmarked configuration silently."""
+    """The launch geometries of the production kernel the benchmark runs: one 32-thread CTA per shard, `warps_per_sm`
+    of them resident per SM.  Pinned so that a planner change cannot move the benchmarked configuration silently."""
     import word2bits_b200 as w2b
     want = {  # (D, window, negative, bitlevel): (slots, queue_entries, warps_per_sm, smem_bytes)
         (800, 10, 24, 1): (4, 128, 12, 17440),   # BASELINE configs[1]

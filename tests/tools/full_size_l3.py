@@ -10,7 +10,7 @@ import word2bits_b200 as w2b
 from oracle import pyoracle as po
 
 tokens = int(sys.argv[1]) if len(sys.argv) > 1 else 3_000_000
-shards = [int(x) for x in sys.argv[2:]] or [16, 148, 1776]
+shards = [int(x) for x in sys.argv[2:]] or [16, 132, 1584]
 cdf, _ = bench.zipf_cdf(400000)
 ids = bench.synth_ids(tokens, 99, cdf)
 path = bench._write_text(ids, os.path.join(tempfile.gettempdir(), "l3_"))

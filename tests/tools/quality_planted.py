@@ -46,7 +46,7 @@ def run(name, exe, extra):
 ref = os.path.join(ROOT, "oracle", "_ref", "word2bits")
 ours = os.path.join(ROOT, "word2bits_b200", "word2bits")
 # python tests/tools/quality_planted.py [shard counts; 0 = the CLI's default, "ref" = the reference at 16 threads]
-which = sys.argv[1:] or ["ref", "0", "16", "148", "2960"]
+which = sys.argv[1:] or ["ref", "0", "16", "132", "2640"]
 for w in which:
     if w == "ref":
         if os.path.exists(ref):

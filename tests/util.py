@@ -1,4 +1,6 @@
-"""Shared helpers for the tests: deterministic synthetic corpora."""
+"""Shared helpers for the tests: deterministic synthetic corpora, digests of the reference's outputs."""
+import hashlib
+import json
 import os
 
 import numpy as np
@@ -29,6 +31,24 @@ def zipf_corpus(path, n_tokens, vocab, seed=0, newline_every=0, tail=True, expon
 
 def bits(a):
     return np.ascontiguousarray(a, np.float32).view(np.uint32)
+
+
+def digest(x):
+    """SHA-256 of an array's bytes (dtype and shape included) or of a list of words."""
+    h = hashlib.sha256()
+    if isinstance(x, list):
+        h.update(json.dumps(x).encode())
+    else:
+        a = np.ascontiguousarray(x)
+        h.update(("%s %s " % (a.dtype.str, a.shape)).encode())
+        h.update(a.tobytes())
+    return h.hexdigest()
+
+
+def reference_outputs(section):
+    """What the unmodified reference computed for a test (tests/golden/make_reference_outputs.py)."""
+    with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_outputs.json")) as f:
+        return json.load(f)[section]
 
 
 def planted_topic_corpus(path, vocab=5000, topics=25, sentences=60000, length=20, p_topic=0.5, seed=7):

@@ -1,5 +1,5 @@
 #!/bin/bash
-# DRAM traffic of the training kernel at the bench's own step size (VERDICT r1 item 8): for each workload, bench.py's
+# DRAM traffic of the training kernel at the bench's own step size (profiles/traffic.json): for each workload, bench.py's
 # resident run under `ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum` (one pass, no replay), the first
 # TIMED step's launch; tools/make_traffic_json.py pairs it with the positions that launch trained.
 #   bash tools/measure_traffic.sh c2 c3 c4      -> gpurun_out/traffic_<w>.csv, gpurun_out/steps_<w>.json

@@ -1,9 +1,9 @@
-// Micro-benchmark (not part of the product): how fast can a B200 stream embedding rows through shared memory with
+// Micro-benchmark (not part of the product): how fast can an H100 stream embedding rows through shared memory with
 // one WARP per stream — cp.async.bulk row in, (optional touch), cp.reduce.async.bulk.add.f32 row back — as a function
 // of warps per SM, ring depth and row size, for Zipf(1.0) and uniform row ids?  This is the skeleton of the
 // warp-per-shard training kernel without its arithmetic: the number it prints is the memory-system ceiling of that
 // design (gather + scatter-add, "algorithmic" bytes = 2 x row bytes per row).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o membench membench.cu && ./membench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o membench membench.cu && ./membench
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>

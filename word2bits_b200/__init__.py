@@ -1,7 +1,7 @@
-"""word2bits_b200 — B200-native Word2Bits training path.
+"""word2bits_b200 — H100-native Word2Bits training path.
 
 Python mirror of the C ABI (include/w2b.h); the compute lives in libw2b.so (hand-written
-sm_100a CUDA) and is driven the same way the C++ CLI (csrc/main.cpp) drives it.
+sm_90a CUDA) and is driven the same way the C++ CLI (csrc/main.cpp) drives it.
 Mirrors the reference's surface: the constructor arguments are its command-line flags
 (src/word2bits.cpp:596-611, same names and defaults)."""
 import ctypes as C

@@ -1,4 +1,4 @@
-// word2bits — drop-in command line for the B200 training path.
+// word2bits — drop-in command line for the H100 training path.
 //
 // Same flags, defaults, progress lines, exit codes and output files as the reference's main()
 // / TrainModel() (src/word2bits.cpp:518-621).  Differences, all additive:
@@ -146,9 +146,8 @@ int main(int argc, char **argv) {
   if (num_threads <= 0) {
     int s = 0;
     if (w2b_suggest_shards(&cfg, &s)) die("w2b_suggest_shards");
-    // every shard is a concurrent Hogwild worker: on a small corpus too many of them cost quality (planted-topic
-    // protocol, 5 M tokens: kNN purity 0.584 reference / 0.576 with 148 shards / 0.548 with 740), so keep at least
-    // ~20 k words per shard; from ~60 M words per GPU on, the GPU is full
+    // every shard is a concurrent Hogwild worker: on a small corpus too many of them cost quality (tests/tools/
+    // quality_planted.py measures kNN purity against the shard count), so keep at least ~20 k words per shard
     s *= ngpus;
     while (s > ngpus && train_words / s < 20000) s /= 2;
     cfg.num_shards = s;

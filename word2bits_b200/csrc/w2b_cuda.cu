@@ -215,7 +215,6 @@ static apply_fn pick_apply(const w2b_ctx *c) {
 typedef void (*warp_fn)(TrainParams, int, int, ApplyArgs);
 // warps (= 1-warp CTAs) per SM the register allocation is sized for; multiples of 4 because the register file is
 // split over the four SM sub-partitions: 12 warps -> 168 registers per thread, 16 -> 128, 20 -> 96, 24 -> 80.
-// Measured (profiles/r02_warp_sweep_more_warps.md): one step denser is 2-11 % slower, except for the narrowest rows.
 // Rows wider than 1024 floats (the reference publishes 1200-dimensional vectors): 8 warps (216 registers) up to
 // 1536 floats, 4 warps (248 registers) up to 2048.
 static int warp_minb_of(int nj) { return nj >= 13 ? 4 : (nj >= 9 ? 8 : (nj >= 5 ? 12 : (nj >= 3 ? 16 : (nj == 2 ? 20 : 24)))); }

@@ -4,7 +4,7 @@
 // (:155) and the arg-max cosine over the whole vocabulary except the three query words
 // (:158-177), first index winning ties and only strictly positive scores counting (bestd
 // starts at 0, :150).  Here all questions are scored together as one Q x V x D contraction
-// on the tensor cores (w2b_eval_tc.cuh: TF32 tcgen05.mma fed by TMA, accumulators in TMEM) used as a FILTER
+// on the tensor cores (w2b_eval_tc.cuh: TF32 wgmma fed by TMA, accumulators in registers) used as a FILTER
 // with a proven error bound, followed by an fp32 re-score of the surviving candidates in the reference's
 // operation order — so the arg-max is the reference's arg-max; the report text is the reference's, line for line.
 #include <cuda_runtime.h>

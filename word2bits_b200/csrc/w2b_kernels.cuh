@@ -1,4 +1,4 @@
-// Device code of the Word2Bits training path for sm_100a.
+// Device code of the Word2Bits training path for sm_90a.
 //
 // One CTA walks one corpus shard exactly like one reference thread does
 // (TrainModelThread, src/word2bits.cpp:363-516): sentence builder + sub-sampling,

@@ -1,4 +1,4 @@
-// PTX wrappers shared by the TMA-staged training kernels (sm_100a): mbarriers, bulk (non-tensor TMA) row copies
+// PTX wrappers shared by the TMA-staged training kernels (sm_90a): mbarriers, bulk (non-tensor TMA) row copies
 // global -> shared, bulk reduce-add shared -> global, async-proxy fence, 128-bit shared-memory accesses.
 // tests/emu compiles the kernels for the host with -DW2B_EMULATE, which swaps these for tests/emu/w2b_emu_ptx.h.
 #pragma once

@@ -1,7 +1,7 @@
-// Production kernel of the Word2Bits training path for sm_100a: one WARP per corpus shard.
+// Production kernel of the Word2Bits training path for sm_90a: one WARP per corpus shard.
 //
 // A shard is what one reference thread walks (TrainModelThread, src/word2bits.cpp:363-516).  Here it is one
-// warp in a CTA of its own (32 threads, grid = shards), so a B200 runs 148 x 12..32 shards side by side and
+// warp in a CTA of its own (32 threads, grid = shards), so an H100 runs 132 x 4..24 shards side by side and
 // hides HBM latency with shards, not with a deep pipeline inside a shard.  The warp does everything the
 // reference thread does, in the reference's order:
 //   * sampling (:379-460): learning-rate schedule, sentence builder + sub-sampling, shard termination, window
@@ -83,12 +83,13 @@ __host__ __device__ inline int warp_queue_capacity(int window, int negative) {
   return q;
 }
 
-// ---------------------------------------------------------------------------- packed fp32 pairs (FFMA2)
+// ---------------------------------------------------------------------------- fp32 pairs
+// (sm_90 has no packed fp32 arithmetic: a pair is two scalar round-to-nearest operations)
 struct F2 { float x, y; };
-#ifdef W2B_EMULATE
 __device__ __forceinline__ F2 fma2(F2 a, F2 b, F2 c) { return F2{fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)}; }
 __device__ __forceinline__ F2 mul2(F2 a, F2 b) { return F2{__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)}; }
 __device__ __forceinline__ F2 add2(F2 a, F2 b) { return F2{__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)}; }
+#ifdef W2B_EMULATE
 __device__ __forceinline__ float sign_level(float x, float level) {  // (x & 0x80000000) | level
   unsigned xi, li;
   memcpy(&xi, &x, 4); memcpy(&li, &level, 4);
@@ -98,31 +99,6 @@ __device__ __forceinline__ float sign_level(float x, float level) {  // (x & 0x8
 }
 __device__ __forceinline__ float ldc_exptab(int i) { return c_exptab[i]; }
 #else
-__device__ __forceinline__ unsigned long long f2_bits(F2 a) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a.x), "f"(a.y));
-  return r;
-}
-__device__ __forceinline__ F2 f2_from(unsigned long long r) {
-  F2 a;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(a.x), "=f"(a.y) : "l"(r));
-  return a;
-}
-__device__ __forceinline__ F2 fma2(F2 a, F2 b, F2 c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(f2_bits(a)), "l"(f2_bits(b)), "l"(f2_bits(c)));
-  return f2_from(d);
-}
-__device__ __forceinline__ F2 mul2(F2 a, F2 b) {
-  unsigned long long d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(f2_bits(a)), "l"(f2_bits(b)));
-  return f2_from(d);
-}
-__device__ __forceinline__ F2 add2(F2 a, F2 b) {
-  unsigned long long d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(f2_bits(a)), "l"(f2_bits(b)));
-  return f2_from(d);
-}
 __device__ __forceinline__ float sign_level(float x, float level) {  // (x & 0x80000000) | level: one LOP3
   unsigned r;
   asm("lop3.b32 %0, %1, 0x80000000, %2, 0xEA;" : "=r"(r) : "r"(__float_as_uint(x)), "r"(__float_as_uint(level)));
@@ -317,10 +293,6 @@ __device__ inline int warp_next_position(const TrainParams &p, const ShardState 
 
 // BM: compile-time bitlevel 0/1/2, 9 = run time.  NJ = float4 columns per lane = ceil(D / 128).  MINB = CTAs (warps)
 // per SM the register allocation is sized for.
-// (Measured alternatives that did not pay on B200, profiles/r02_warp_sweep_*.md: scatter-adds through the load/store
-// unit — red.global.add.v4.f32 from registers — instead of the bulk-copy engine: same throughput, same memory-system
-// ceiling; 16 / 20 / 24 instead of 12 / 16 / 20 warps per SM: 2-11 % slower except for rows of <= 128 floats; 2 or 3
-// bulk-reduce groups left pending instead of 1: no change.)
 // REG = 1: -reg != 0 (:443-445,:471,:490,:501).  Every row then also decays by 2*alpha*reg times its own (raw) value:
 // a target row in the same scatter as its update (g*context_avg - 2*alpha*reg*v), a context row by a scatter of its
 // own when it is read (the reference subtracts at the end of the position from a value this thread has not changed
