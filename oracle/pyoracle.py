@@ -58,6 +58,7 @@ def lib():
         L = C.CDLL(path)
         L.w2bo_quantize.restype = C.c_float
         L.w2bo_quantize.argtypes = [C.c_float, C.c_int]
+        L.w2bo_quantize_n.argtypes = [_f32p, _f32p, C.c_int64, C.c_int]
         L.w2bo_sigmoid.restype = C.c_float
         L.w2bo_sigmoid.argtypes = [C.c_float]
         L.w2bo_lcg.restype = C.c_uint64
@@ -94,13 +95,11 @@ def lib():
 
 
 def quantize(x, b):
-    L = lib()
     x = np.asarray(x, dtype=np.float32)
-    out = np.empty_like(x)
-    flat_in, flat_out = x.ravel(), out.ravel()
-    for i in range(flat_in.size):
-        flat_out[i] = L.w2bo_quantize(float(flat_in[i]), int(b))
-    return out
+    flat = np.ascontiguousarray(x.ravel())
+    out = np.empty_like(flat)
+    lib().w2bo_quantize_n(flat, out, flat.size, int(b))
+    return out.reshape(x.shape)
 
 
 def exptable():

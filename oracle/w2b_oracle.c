@@ -32,6 +32,10 @@ float w2bo_quantize(float x, int b) {
   return sgn * level;
 }
 
+void w2bo_quantize_n(const float *x, float *out, int64_t n, int b) {
+  for (int64_t i = 0; i < n; i++) out[i] = w2bo_quantize(x[i], b);
+}
+
 /* :67-71 */
 float w2bo_sigmoid(float x) {
   if (x > 6) return 1;

@@ -24,6 +24,7 @@ extern "C" {
 
 /* ---- scalar pieces -------------------------------------------------------------- */
 float w2bo_quantize(float x, int bitlevel);           /* :73-108 */
+void w2bo_quantize_n(const float *x, float *out, int64_t n, int bitlevel); /* w2bo_quantize per element */
 float w2bo_sigmoid(float x);                          /* :67-71  */
 uint64_t w2bo_lcg(uint64_t r);                        /* :352 et al. */
 void w2bo_exptable(float *out /*1000*/);              /* :614-618 */

@@ -421,3 +421,18 @@ def test_default_geometry_is_the_measured_one():
         p = w2b.warp_plan(size=D, window=W, negative=neg, bitlevel=b, vocab_size=400001)
         assert p["warp"] == 1
         assert (p["slots"], p["queue_entries"], p["warps_per_sm"], p["smem_bytes"]) == geo, (D, p)
+
+
+def test_wide_register_kernels_fit_1024_threads():
+    """The register kernel runs one thread per column group, up to 1024 per CTA (D = 4096).  The instantiations the
+    dispatch launches at that width (strict mode always; fast mode when the speed-tuned ones cannot take a row's
+    threads) must hold at most 64 registers per thread: 1024 x 64 is the register file of an SM."""
+    import shutil
+    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    if not os.path.exists(tool):
+        pytest.skip("cuobjdump not available")
+    out = subprocess.run([tool, "--dump-resource-usage", LIB], capture_output=True, text=True, check=True).stdout
+    regs = {m.group(1): int(m.group(2)) for m in re.finditer(r"Function (\S+):\s+REG:(\d+)", out)}
+    wide = {k: r for k, r in regs.items() if "train_shards_wide_kernel" in k or "apply_position_wide_kernel" in k}
+    assert len(wide) == 12, sorted(wide)  # {train, apply} x {VEC 4, VEC 1} x {fast, fast -reg, strict}
+    assert all(r <= 64 for r in wide.values()), wide

@@ -109,6 +109,7 @@ struct w2b_ctx {
   int nlocal = 0;  // shards owned by this context
   long long pitch = 0;  // floats per row of u / v: layer1_size rounded up to a multiple of 4 (bulk copies move 16-byte units)
   int vec = 4, ncol = 0, threads = 0, group = 9;
+  bool wide_train = false, wide_apply = false;  // register kernel: the 1024-thread (64-register) instantiations
   bool warp = false;       // production warp-per-shard kernel (csrc/w2b_warp.cuh) usable for this configuration
   int warp_k = 0, warp_qcap = 0, warp_minb = 0;  // ring slots per warp, job queue entries, warps per SM
   int warp_sen_smem = 1;   // the sentence buffer fits shared memory (else d_sen)
@@ -179,12 +180,20 @@ template <int VEC, int BM, bool REG, bool STRICT, int G>
 static train_fn tk() { return train_shards_kernel<VEC, BM, REG, STRICT, G>; }
 template <int VEC, int BM, bool REG, bool STRICT, int G>
 static apply_fn ak() { return apply_position_kernel<VEC, BM, REG, STRICT, G>; }
+template <int VEC, bool REG, bool STRICT, int G>
+static train_fn tk_wide() { return train_shards_wide_kernel<VEC, 9, REG, STRICT, G>; }
+template <int VEC, bool REG, bool STRICT, int G>
+static apply_fn ak_wide() { return apply_position_wide_kernel<VEC, 9, REG, STRICT, G>; }
 
 static int bm_of(int bits) { return (bits == 0 || bits == 1 || bits == 2) ? bits : 9; }
 
 static train_fn pick_train(const w2b_ctx *c) {
   const bool reg = c->cfg.reg != 0.f;
-  if (c->cfg.mode == W2B_MODE_STRICT) return c->vec == 4 ? tk<4, 9, true, true, 1>() : tk<1, 9, true, true, 1>();
+  if (c->cfg.mode == W2B_MODE_STRICT) return c->vec == 4 ? tk_wide<4, true, true, 1>() : tk_wide<1, true, true, 1>();
+  if (c->wide_train) {
+    if (c->vec == 1) return reg ? tk_wide<1, true, false, 5>() : tk_wide<1, false, false, 5>();
+    return reg ? tk_wide<4, true, false, 5>() : tk_wide<4, false, false, 5>();
+  }
   if (c->vec == 1) return reg ? tk<1, 9, true, false, 9>() : tk<1, 9, false, false, 9>();
   const int bm = bm_of(c->cfg.bitlevel);
 #define W2B_PICK(BM)                                                         \
@@ -201,7 +210,11 @@ static train_fn pick_train(const w2b_ctx *c) {
 
 static apply_fn pick_apply(const w2b_ctx *c) {
   const bool reg = c->cfg.reg != 0.f;
-  if (c->cfg.mode == W2B_MODE_STRICT) return c->vec == 4 ? ak<4, 9, true, true, 1>() : ak<1, 9, true, true, 1>();
+  if (c->cfg.mode == W2B_MODE_STRICT) return c->vec == 4 ? ak_wide<4, true, true, 1>() : ak_wide<1, true, true, 1>();
+  if (c->wide_apply) {
+    if (c->vec == 1) return reg ? ak_wide<1, true, false, 5>() : ak_wide<1, false, false, 5>();
+    return reg ? ak_wide<4, true, false, 5>() : ak_wide<4, false, false, 5>();
+  }
   if (c->vec == 1) return reg ? ak<1, 9, true, false, 9>() : ak<1, 9, false, false, 9>();
   const int bm = bm_of(c->cfg.bitlevel);
 #define W2B_PICK(BM)                                                         \
@@ -306,6 +319,29 @@ static void plan_warp(w2b_ctx *c) {
   c->warp_smem = warp_layout(pitch, K, qcap, sen_smem).total;
 }
 
+// Register kernel (configurations the warp kernel does not take): c->threads threads per CTA.  The instantiations
+// compiled for speed run when they can take that many threads; otherwise the wide ones (__launch_bounds__(1024)).
+// A width that not even those can serve is refused here, at creation, instead of failing at its first launch.
+static int plan_register_kernel(w2b_ctx *c) {
+  c->wide_train = c->wide_apply = false;
+  cudaFuncAttributes fa;
+  if (c->cfg.mode != W2B_MODE_STRICT) {
+    CK(cudaFuncGetAttributes(&fa, (const void *)pick_train(c)));
+    c->wide_train = c->threads > fa.maxThreadsPerBlock;
+    CK(cudaFuncGetAttributes(&fa, (const void *)pick_apply(c)));
+    c->wide_apply = c->threads > fa.maxThreadsPerBlock;
+  }
+  for (const void *fn : {(const void *)pick_train(c), (const void *)pick_apply(c)}) {
+    CK(cudaFuncGetAttributes(&fa, fn));
+    if (c->threads > fa.maxThreadsPerBlock) {
+      w2b_set_error("layer1_size %lld needs %d threads per CTA; the register kernel takes at most %d for this "
+                    "configuration", (long long)c->cfg.layer1_size, c->threads, fa.maxThreadsPerBlock);
+      return W2B_EINVAL;
+    }
+  }
+  return W2B_OK;
+}
+
 static size_t dyn_smem(const w2b_ctx *c) {
   return c->cfg.mode == W2B_MODE_STRICT ? (size_t)c->cfg.layer1_size * sizeof(float) : 0;
 }
@@ -369,10 +405,12 @@ static int validate(const w2b_config *c) {
   if (c->plain_store != 0) { w2b_set_error("plain_store: the racy load/add/store variant was removed; must be 0"); return W2B_EINVAL; }
   const long long D = c->layer1_size;
   // production kernel: any D <= 2048 (rows padded to whole float4s); register kernel: D <= 4096 when divisible by 4
-  // (a thread per float4), else D <= 1024 (a thread per float) — strict mode and kernel = 1 always run the latter
+  // (a thread per float4), else D <= 1024 (a thread per float) — strict mode and kernel = 1 always run the latter.
+  // Every width accepted here launches (the wide instantiations, plan_register_kernel).
   const bool reg_kernel = c->mode == W2B_MODE_STRICT || c->kernel == 1 || D > 2048;
   if (D > 4096 || (reg_kernel && D % 4 != 0 && D > 1024)) {
-    w2b_set_error("layer1_size %lld unsupported (max 2048; 4096 when divisible by 4; strict mode / kernel 1: 1024 unless divisible by 4)", D);
+    w2b_set_error("layer1_size %lld unsupported (at most 4096; in strict mode, with kernel 1 and above 2048 it must "
+                  "also be divisible by 4 when above 1024)", D);
     return W2B_EINVAL;
   }
   return W2B_OK;
@@ -394,6 +432,10 @@ extern "C" int w2b_suggest_shards(const w2b_config *cfg, int *out) {
   CK(cudaGetDeviceProperties(&prop, cfg->device));
   int per_sm = 0;
   plan_warp(&tmp);
+  if (!tmp.warp) {
+    rc = plan_register_kernel(&tmp);
+    if (rc) return rc;
+  }
   if (tmp.warp) {
     warp_fn wf = pick_warp(&tmp);
     CK(cudaFuncSetAttribute(wf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tmp.warp_smem));
@@ -483,6 +525,10 @@ static int create_impl(const w2b_config *cfg, w2b_ctx **out) {
   if (c->group != 5 && c->group != 9 && c->group != 13) c->group = 9;  // register kernel instantiations
   plan_warp(c);
   CK(cudaSetDevice(cfg->device));
+  if (!c->warp) {
+    rc = plan_register_kernel(c);
+    if (rc) return rc;
+  }
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
   c->sm_count = prop.multiProcessorCount;

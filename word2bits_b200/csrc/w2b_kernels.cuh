@@ -487,7 +487,7 @@ __device__ __forceinline__ void process_position(const TrainParams &p, const Pos
 
 // ----------------------------------------------------------------------- shard kernel
 template <int VEC, int BM, bool HAS_REG, bool STRICT, int G>
-__global__ void train_shards_kernel(TrainParams p) {
+__device__ __forceinline__ void train_shards(TrainParams p) {
   extern __shared__ float dyn[];  // strict mode: D floats
   __shared__ int s_sen[kMaxS];
   __shared__ PosDesc s_desc[2];
@@ -604,10 +604,20 @@ __global__ void train_shards_kernel(TrainParams p) {
   }
 }
 
+// A CTA has one thread per column group (ceil(D / VEC) of them, up to 1024).  train_shards_kernel is compiled for
+// speed and holds more registers than 1024 threads may have (up to 182 per thread: 352 threads); the wide copy is
+// held to 64 registers so that every width the ABI accepts launches.  Strict mode always runs the wide copy.
+template <int VEC, int BM, bool HAS_REG, bool STRICT, int G>
+__global__ void train_shards_kernel(TrainParams p) { train_shards<VEC, BM, HAS_REG, STRICT, G>(p); }
+template <int VEC, int BM, bool HAS_REG, bool STRICT, int G>
+__global__ void __launch_bounds__(1024, 1) train_shards_wide_kernel(TrainParams p) {
+  train_shards<VEC, BM, HAS_REG, STRICT, G>(p);
+}
+
 // One explicit position (L1 single-step parity hook).
 template <int VEC, int BM, bool HAS_REG, bool STRICT, int G>
-__global__ void apply_position_kernel(TrainParams p, const int *ctx, int cw, const int *tg, int nt, float *f_out,
-                                      double *loss_out) {
+__device__ __forceinline__ void apply_position(TrainParams p, const int *ctx, int cw, const int *tg, int nt,
+                                               float *f_out, double *loss_out) {
   extern __shared__ float dyn[];
   __shared__ PosDesc s_desc;
   __shared__ BlockScratch s_bs;
@@ -634,6 +644,17 @@ __global__ void apply_position_kernel(TrainParams p, const int *ctx, int cw, con
     for (int o = 16; o > 0; o >>= 1) loss += __shfl_xor_sync(kFull, loss, o);
   }
   if (threadIdx.x == 0 && loss_out) *loss_out = loss;
+}
+template <int VEC, int BM, bool HAS_REG, bool STRICT, int G>
+__global__ void apply_position_kernel(TrainParams p, const int *ctx, int cw, const int *tg, int nt, float *f_out,
+                                      double *loss_out) {
+  apply_position<VEC, BM, HAS_REG, STRICT, G>(p, ctx, cw, tg, nt, f_out, loss_out);
+}
+template <int VEC, int BM, bool HAS_REG, bool STRICT, int G>
+__global__ void __launch_bounds__(1024, 1) apply_position_wide_kernel(TrainParams p, const int *ctx, int cw,
+                                                                      const int *tg, int nt, float *f_out,
+                                                                      double *loss_out) {
+  apply_position<VEC, BM, HAS_REG, STRICT, G>(p, ctx, cw, tg, nt, f_out, loss_out);
 }
 
 // ------------------------------------------------------------------- auxiliary kernels
