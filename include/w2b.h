@@ -219,6 +219,15 @@ typedef struct {
 } w2b_accuracy;
 int w2b_compute_accuracy(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file,
                          int device, w2b_accuracy *acc, char *report, int64_t report_cap);
+/* The same evaluation, per question: answers[i] = index of the word chosen for the i-th question of the file (every
+ * question line counts, in file order), -1 when the question is skipped (a word is not in the vocabulary) or no word
+ * scores above 0.  At most answers_cap are written; *n_questions = the number of questions. */
+int w2b_analogy_answers(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file,
+                        int device, int32_t *answers, int64_t answers_cap, int64_t *n_questions);
+/* Test hook of the tensor-core filter: approx[q*words + c] = its TF32 score of Q row q against M row c (both used as
+ * given, D floats per row), eps[q] = the error bound it uses for question q (eps may be NULL). */
+int w2b_eval_filter_scores(const float *Q, int64_t nq, const float *M, int64_t words, int64_t D, int device,
+                           float *approx, float *eps);
 
 /* Multi-GPU replica averaging (SURVEY §8(e)); G=1 contexts never touch NCCL. */
 int w2b_device_ptrs(w2b_ctx *ctx, void **u, void **v, int64_t *elems);

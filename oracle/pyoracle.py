@@ -90,6 +90,10 @@ def lib():
         L.w2bo_export.argtypes = [C.POINTER(Model), _f32p]
         L.w2bo_write_vectors.restype = C.c_int
         L.w2bo_write_vectors.argtypes = [C.POINTER(Model), C.c_void_p, C.c_char_p, C.c_int]
+        L.w2bo_analogy_normalize.argtypes = [_f32p, C.c_int64, C.c_int64, C.c_int, C.c_int]
+        L.w2bo_analogy.restype = C.c_int
+        L.w2bo_analogy.argtypes = [C.c_char_p, C.c_int, C.c_int64, C.c_char_p, C.c_int, C.c_int, C.c_char_p,
+                                   C.c_int64, _i32p, C.c_int64, C.POINTER(C.c_int64)]
         _lib = L
     return _lib
 
@@ -100,6 +104,30 @@ def quantize(x, b):
     out = np.empty_like(flat)
     lib().w2bo_quantize_n(flat, out, flat.size, int(b))
     return out.reshape(x.shape)
+
+
+AN_FUSED, AN_LANE_NORM = 1, 2  # negative controls of the analogy evaluator (w2b_oracle.h)
+
+
+def analogy_normalize(M, bits, flags=0):
+    """compute-accuracy.c :106-110 on a copy of M (words x D): quantize, then divide by the row's length."""
+    M = np.array(M, np.float32, order="C", copy=True)
+    lib().w2bo_analogy_normalize(M.reshape(-1), M.shape[0], M.shape[1], int(bits), int(flags))
+    return M
+
+
+def analogy(vectors_file, questions_file, bitlevel=0, threshold=0, flags=0, threads=None):
+    """src/compute-accuracy.c on the CPU: (report text, int32 array of the chosen word per question in file order,
+    -1 where the question is skipped or no word scores above 0)."""
+    threads = threads or min(32, os.cpu_count() or 1)
+    buf = C.create_string_buffer(1 << 22)
+    ans = np.empty(os.path.getsize(questions_file) // 4 + 1, np.int32)  # a question takes at least 4 bytes
+    n = C.c_int64()
+    rc = lib().w2bo_analogy(vectors_file.encode(), int(bitlevel), int(threshold), questions_file.encode(),
+                            int(flags), int(threads), buf, len(buf), ans, len(ans), C.byref(n))
+    if rc:
+        raise OSError("w2bo_analogy failed (%d) on %s / %s" % (rc, vectors_file, questions_file))
+    return buf.value.decode("latin1"), ans[: n.value].copy()
 
 
 def exptable():

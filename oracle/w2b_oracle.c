@@ -532,3 +532,236 @@ int w2bo_write_vectors(const w2bo_model *m, const w2bo_corpus *c, const char *pa
   fclose(fo);
   return 0;
 }
+
+/* ============================================================ analogy evaluator
+ * src/compute-accuracy.c of the reference, with the floating-point operations of the build the stored reports come
+ * from (gcc -O3 -march=x86-64-v3, oracle/Makefile).  Its compute-accuracy quantize() is the same function as
+ * w2bo_quantize() (bit level 3 gives +-0, NaN takes the + sign).  Two orders are not what the C text suggests:
+ *   len += M*M (:108)   the loop is split at 4*floor(D/4): the squares before it are rounded on their own (vmulps)
+ *                       and added one by one in index order (vaddss); the last D mod 4 terms are fused (vfmadd231ss);
+ *   dist += vec*M (:164) a rounded product, then a rounded add (vmulss, vaddss), in index order: never fused.
+ * W2BO_AN_FUSED and W2BO_AN_LANE_NORM swap in other orders; tests use them to show the pin would notice. */
+#include <ctype.h>
+
+#define AN_MAX_W 50      /* :24 */
+#define AN_MAX_SIZE 2000 /* :22 */
+
+void w2bo_analogy_normalize(float *M, int64_t words, int64_t D, int bitlevel, int flags) {
+  for (int64_t b = 0; b < words; b++) {
+    float *r = M + b * D;
+    for (int64_t a = 0; a < D; a++) r[a] = w2bo_quantize(r[a], bitlevel); /* :106 */
+    float len = 0;
+    if (flags & W2BO_AN_LANE_NORM) {
+      /* 32 lane-strided fused partial sums, then an xor butterfly (what the GPU normalised with before) */
+      float s[32];
+      for (int l = 0; l < 32; l++) {
+        s[l] = 0;
+        for (int64_t a = l; a < D; a += 32) s[l] = fmaf(r[a], r[a], s[l]);
+      }
+      for (int o = 16; o > 0; o >>= 1) {
+        float t[32];
+        for (int l = 0; l < 32; l++) t[l] = s[l] + s[l ^ o];
+        memcpy(s, t, sizeof s);
+      }
+      len = s[0];
+    } else {
+      const int64_t D4 = D & ~(int64_t)3;
+      for (int64_t a = 0; a < D4; a++) {
+        const float p = r[a] * r[a];
+        len = len + p;
+      }
+      for (int64_t a = D4; a < D; a++) len = fmaf(r[a], r[a], len);
+    }
+    len = sqrtf(len); /* :109, correctly rounded either way */
+    for (int64_t a = 0; a < D; a++) r[a] = r[a] / len; /* :110: a zero row becomes NaN */
+  }
+}
+
+typedef struct {
+  const float *M;
+  int64_t words, D;
+  const int64_t *q; /* b1, b2, b3 per scored question */
+  int32_t *best;
+  int64_t nq;
+  int flags, nthreads, id;
+} an_job;
+
+static void *an_worker(void *p) {
+  an_job *j = (an_job *)p;
+  const int64_t D = j->D;
+  float *vec = (float *)malloc(sizeof(float) * (size_t)(D ? D : 1));
+  for (int64_t i = j->id; i < j->nq; i += j->nthreads) {
+    const int64_t b1 = j->q[3 * i], b2 = j->q[3 * i + 1], b3 = j->q[3 * i + 2];
+    for (int64_t a = 0; a < D; a++) vec[a] = (j->M[a + b2 * D] - j->M[a + b1 * D]) + j->M[a + b3 * D]; /* :155 */
+    float bestd = 0; /* :146 */
+    int32_t bestc = -1;
+    for (int64_t c = 0; c < j->words; c++) { /* :158-177 */
+      if (c == b1 || c == b2 || c == b3) continue;
+      const float *m = j->M + c * D;
+      float dist = 0;
+      if (j->flags & W2BO_AN_FUSED) {
+        for (int64_t a = 0; a < D; a++) dist = fmaf(vec[a], m[a], dist);
+      } else {
+        for (int64_t a = 0; a < D; a++) {
+          const float p = vec[a] * m[a];
+          dist = dist + p;
+        }
+      }
+      if (dist > bestd) { bestd = dist; bestc = (int32_t)c; }
+    }
+    j->best[i] = bestc;
+  }
+  free(vec);
+  return NULL;
+}
+
+typedef struct { char *p; int64_t n, cap; } an_text;
+static void an_printf(an_text *t, const char *fmt, ...) __attribute__((format(printf, 2, 3)));
+#include <stdarg.h>
+static void an_printf(an_text *t, const char *fmt, ...) {
+  char line[4096];
+  va_list ap;
+  va_start(ap, fmt);
+  int k = vsnprintf(line, sizeof line, fmt, ap);
+  va_end(ap);
+  if (k < 0) return;
+  if (k >= (int)sizeof line) k = (int)sizeof line - 1;
+  if (t->n + k + 1 > t->cap) {
+    t->cap = (t->n + k + 1) * 2;
+    t->p = (char *)realloc(t->p, (size_t)t->cap);
+  }
+  memcpy(t->p + t->n, line, (size_t)k + 1);
+  t->n += k;
+}
+
+static void an_upper(char *s) {
+  for (size_t a = 0; a < strlen(s); a++) s[a] = (char)toupper((unsigned char)s[a]);
+}
+
+int w2bo_analogy(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file, int flags,
+                 int nthreads, char *report, int64_t report_cap, int32_t *answers, int64_t answers_cap,
+                 int64_t *n_questions) {
+  FILE *f = fopen(vectors_file, "rb");
+  if (!f) return 1;
+  long long words = 0, size = 0;
+  if (fscanf(f, "%lld", &words) != 1) { fclose(f); return 2; } /* :85-87 */
+  if (threshold) if (words > threshold) words = threshold;
+  if (fscanf(f, "%lld", &size) != 1 || words < 1 || size < 1) { fclose(f); return 2; }
+  char *vocab = (char *)calloc((size_t)(words + 1) * AN_MAX_W, 1);
+  float *M = (float *)malloc(sizeof(float) * (size_t)words * (size_t)size);
+  for (long long b = 0; b < words; b++) { /* :96-105 */
+    long long a = 0;
+    for (;;) {
+      vocab[b * AN_MAX_W + a] = (char)fgetc(f);
+      if (feof(f) || vocab[b * AN_MAX_W + a] == ' ') break;
+      if (a < AN_MAX_W && vocab[b * AN_MAX_W + a] != '\n') a++;
+    }
+    vocab[b * AN_MAX_W + a] = 0;
+    for (a = 0; a < AN_MAX_W; a++) vocab[b * AN_MAX_W + a] = (char)toupper((unsigned char)vocab[b * AN_MAX_W + a]);
+    if (fread(M + b * size, sizeof(float), (size_t)size, f) != (size_t)size) { fclose(f); free(vocab); free(M); return 3; }
+  }
+  fclose(f);
+  w2bo_analogy_normalize(M, words, size, bitlevel, flags); /* :106-110 */
+
+  /* the question loop (:113-186), run twice: first to collect the questions, then to replay the counters */
+  FILE *qf = fopen(questions_file, "rb");
+  if (!qf) { free(vocab); free(M); return 1; }
+  typedef struct { int kind; char name[AN_MAX_SIZE]; int64_t b1, b2, b3; char st4[AN_MAX_SIZE]; int64_t qi; } ev;
+  int64_t nev = 0, evcap = 64, nq = 0, qcap = 64;
+  ev *evs = (ev *)malloc(sizeof(ev) * (size_t)evcap);
+  int64_t *q = (int64_t *)malloc(sizeof(int64_t) * 3 * (size_t)qcap);
+  char st1[AN_MAX_SIZE] = "", st2[AN_MAX_SIZE] = "", st3[AN_MAX_SIZE] = "", st4[AN_MAX_SIZE] = "";
+#define AN_SCAN(s) do { if (fscanf(qf, "%1999s", s) != 1) {} } while (0)
+#define AN_FIND(s, out) do { for (out = 0; out < words; out++) if (!strcmp(&vocab[out * AN_MAX_W], s)) break; } while (0)
+  for (;;) {
+    if (nev == evcap) { evcap *= 2; evs = (ev *)realloc(evs, sizeof(ev) * (size_t)evcap); }
+    ev *e = evs + nev;
+    memset(e, 0, sizeof *e);
+    e->qi = -1;
+    AN_SCAN(st1);
+    an_upper(st1);
+    if (!strcmp(st1, ":") || !strcmp(st1, "EXIT") || feof(qf)) {
+      e->kind = 0;
+      AN_SCAN(st1);
+      e->b1 = feof(qf) ? 1 : 0; /* the stream ended: stop after the counters */
+      strcpy(e->name, st1);
+      nev++;
+      if (e->b1) break;
+      continue;
+    }
+    AN_SCAN(st2); an_upper(st2);
+    AN_SCAN(st3); an_upper(st3);
+    AN_SCAN(st4); an_upper(st4);
+    e->kind = 1;
+    strcpy(e->st4, st4);
+    int64_t b1, b2, b3, b4;
+    AN_FIND(st1, b1); AN_FIND(st2, b2); AN_FIND(st3, b3);
+    e->b1 = b1; e->b2 = b2; e->b3 = b3;
+    if (b1 != words && b2 != words && b3 != words) {
+      AN_FIND(st4, b4);
+      if (b4 != words) {
+        if (nq == qcap) { qcap *= 2; q = (int64_t *)realloc(q, sizeof(int64_t) * 3 * (size_t)qcap); }
+        q[3 * nq] = b1; q[3 * nq + 1] = b2; q[3 * nq + 2] = b3;
+        e->qi = nq++;
+      }
+    }
+    nev++;
+  }
+#undef AN_SCAN
+#undef AN_FIND
+  fclose(qf);
+
+  int32_t *best = (int32_t *)malloc(sizeof(int32_t) * (size_t)(nq ? nq : 1));
+  if (nthreads < 1) nthreads = 1;
+  pthread_t *th = (pthread_t *)malloc(sizeof(pthread_t) * (size_t)nthreads);
+  an_job *jobs = (an_job *)malloc(sizeof(an_job) * (size_t)nthreads);
+  for (int i = 0; i < nthreads; i++) {
+    jobs[i] = (an_job){M, words, size, q, best, nq, flags, nthreads, i};
+    pthread_create(&th[i], NULL, an_worker, &jobs[i]);
+  }
+  for (int i = 0; i < nthreads; i++) pthread_join(th[i], NULL);
+
+  an_text out = {NULL, 0, 0};
+  an_printf(&out, "Starting eval...\n");
+  int TCN = 0, CCN = 0, TACN = 0, CACN = 0, SECN = 0, SYCN = 0, SEAC = 0, SYAC = 0, QID = 0, TQ = 0, TQS = 0;
+  int64_t na = 0;
+  for (int64_t i = 0; i < nev; i++) {
+    const ev *e = evs + i;
+    if (e->kind == 0) {
+      if (TCN == 0) TCN = 1;
+      if (QID != 0) {
+        an_printf(&out, "ACCURACY TOP1: %.2f %%  (%d / %d)\n", CCN / (float)TCN * 100, CCN, TCN);
+        an_printf(&out, "Total accuracy: %.2f %%   Semantic accuracy: %.2f %%   Syntactic accuracy: %.2f %% \n",
+                  CACN / (float)TACN * 100, SEAC / (float)SECN * 100, SYAC / (float)SYCN * 100);
+      }
+      QID++;
+      if (e->b1) break;
+      an_printf(&out, "%s:\n", e->name);
+      TCN = 0;
+      CCN = 0;
+      continue;
+    }
+    TQ++;
+    const int32_t c = e->qi >= 0 ? best[e->qi] : -1;
+    if (answers && na < answers_cap) answers[na] = c;
+    na++;
+    if (e->qi < 0) continue;
+    TQS++;
+    if (c >= 0 && !strcmp(e->st4, &vocab[(int64_t)c * AN_MAX_W])) {
+      CCN++;
+      CACN++;
+      if (QID <= 5) SEAC++; else SYAC++;
+    }
+    if (QID <= 5) SECN++; else SYCN++;
+    TCN++;
+    TACN++;
+  }
+  an_printf(&out, "Questions seen / total: %d %d   %.2f %% \n", TQS, TQ, TQS / (float)TQ * 100);
+  if (report && report_cap > 0) {
+    strncpy(report, out.p, (size_t)report_cap - 1);
+    report[report_cap - 1] = 0;
+  }
+  if (n_questions) *n_questions = na;
+  free(out.p); free(best); free(th); free(jobs); free(evs); free(q); free(vocab); free(M);
+  return 0;
+}

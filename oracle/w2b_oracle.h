@@ -93,6 +93,18 @@ void w2bo_export(const w2bo_model *m, float *out);
 /* Writes the vector file (:560-576). */
 int w2bo_write_vectors(const w2bo_model *m, const w2bo_corpus *c, const char *path, int binary);
 
+/* ---- analogy evaluator (src/compute-accuracy.c, fp32 operation order of its -O3 x86-64-v3 build) ---------- */
+#define W2BO_AN_FUSED 1     /* negative control: fused multiply-add scoring */
+#define W2BO_AN_LANE_NORM 2 /* negative control: 32 lane-strided fused partial sums + butterfly for |row| */
+/* quantize + L2-normalise words rows of D in place (:106-110). */
+void w2bo_analogy_normalize(float *M, int64_t words, int64_t D, int bitlevel, int flags);
+/* The whole program on a vector file and a question file: its report text (stdout) into report, and per question
+ * in file order the chosen word index, or -1 when the question is skipped or no word scores above 0.  flags = 0 is
+ * the reference; nthreads threads share the questions.  Returns 0, or non-zero if a file cannot be read. */
+int w2bo_analogy(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file, int flags,
+                 int nthreads, char *report, int64_t report_cap, int32_t *answers, int64_t answers_cap,
+                 int64_t *n_questions);
+
 #ifdef __cplusplus
 }
 #endif

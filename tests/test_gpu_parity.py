@@ -576,9 +576,9 @@ def _analogy_fixture(tmp_path, D=48, pairs=300, sections=8, per_section=120, bit
 
 @pytest.mark.parametrize("bits,threshold", [(0, 0), (0, 700), (2, 0), (1, 0)])
 def test_gpu_analogy_evaluator_matches_reference(tmp_path, bits, threshold):
-    """SURVEY 8(f).2: the GPU evaluator prints what src/compute-accuracy.c prints.  fp32 vectors:
-    the report is identical text; 1-/2-bit vectors produce exact score ties whose winner depends on
-    the summation order even inside the reference, so the counters are held to +-2 %."""
+    """SURVEY 8(f).2: the GPU evaluator prints what src/compute-accuracy.c prints, identical text for fp32 and for
+    1-/2-bit vectors alike: exact score ties on quantized vectors are broken the reference's way because the scores
+    are computed in the reference's fp32 operation order (tests/test_gpu_evaluator.py checks every answer)."""
     import subprocess
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     vf, qf = _analogy_fixture(tmp_path, bits=bits)
@@ -588,19 +588,9 @@ def test_gpu_analogy_evaluator_matches_reference(tmp_path, bits, threshold):
                          stdin=open(qf), capture_output=True, text=True).stdout
     assert cli == got
     assert acc["questions_total"] == 8 * 120 and acc["questions_seen"] > 0
+    assert got == want
     if bits == 0:
-        assert got == want
         assert acc["correct"] > 0.3 * acc["questions_seen"]   # the planted offsets are recoverable
-    else:
-        import re
-        def nums(txt):
-            return [float(x) for x in re.findall(r"[-+]?\d+\.\d+|\d+", txt)]
-        gw, gg = nums(want), nums(got)
-        assert len(gw) == len(gg) and want.splitlines()[1] == got.splitlines()[1]
-        assert want.splitlines()[-1] == got.splitlines()[-1]          # questions seen / total: exact
-        total_w = [l for l in want.splitlines() if l.startswith("Total accuracy")][-1]
-        total_g = [l for l in got.splitlines() if l.startswith("Total accuracy")][-1]
-        assert abs(nums(total_w)[0] - nums(total_g)[0]) <= 2.0, (total_w, total_g)
 
 
 @pytest.mark.parametrize("D,bits,vocab", [(200, 1, 30000), (72, 0, 9000), (800, 2, 6000), (130, 0, 700)])

@@ -5,6 +5,7 @@ sm_90a CUDA) and is driven the same way the C++ CLI (csrc/main.cpp) drives it.
 Mirrors the reference's surface: the constructor arguments are its command-line flags
 (src/word2bits.cpp:596-611, same names and defaults)."""
 import ctypes as C
+import os
 
 import numpy as np
 
@@ -12,7 +13,7 @@ from . import _lib
 from ._lib import MODE_FAST, MODE_STRICT, TABLE_SIZE, W2BError, check, lib, ptr
 
 __all__ = ["Corpus", "Trainer", "W2BError", "MODE_FAST", "MODE_STRICT", "device_count", "read_packed", "nccl_unique_id",
-           "compute_accuracy", "host_unigram_bounds", "host_exptable", "host_keep_thresholds", "host_lcg_tables", "warp_plan"]
+           "compute_accuracy", "analogy_answers", "eval_filter_scores", "host_unigram_bounds", "host_exptable", "host_keep_thresholds", "host_lcg_tables", "warp_plan"]
 
 
 def device_count():
@@ -303,3 +304,24 @@ def compute_accuracy(vectors_file, questions_file, bitlevel=0, threshold=0, devi
     check(lib.w2b_compute_accuracy(vectors_file.encode(), int(bitlevel), int(threshold), questions_file.encode(),
                                    int(device), C.byref(acc), buf, len(buf)))
     return buf.value.decode("latin1"), {k: getattr(acc, k) for k, _ in acc._fields_}
+
+
+def analogy_answers(vectors_file, questions_file, bitlevel=0, threshold=0, device=0):
+    """Per question of questions_file, in file order: the index of the word compute_accuracy chooses, or -1 (the
+    question is skipped, or no word scores above 0).  int32 numpy array."""
+    ans = np.empty(os.path.getsize(questions_file) // 4 + 1, np.int32)  # a question takes at least 4 bytes
+    n = C.c_int64()
+    check(lib.w2b_analogy_answers(vectors_file.encode(), int(bitlevel), int(threshold), questions_file.encode(),
+                                  int(device), ptr(ans), len(ans), C.byref(n)))
+    return ans[: n.value].copy()
+
+
+def eval_filter_scores(Q, M, device=0):
+    """Test hook: (approx, eps) of the evaluator's tensor-core filter for float32 rows Q (nq x D) and M (words x D):
+    approx[q, c] its TF32 score, eps[q] the error bound it assumes for question q (rows of M of length <= 1)."""
+    Q = np.ascontiguousarray(Q, np.float32)
+    M = np.ascontiguousarray(M, np.float32)
+    approx = np.empty((Q.shape[0], M.shape[0]), np.float32)
+    eps = np.empty(Q.shape[0], np.float32)
+    check(lib.w2b_eval_filter_scores(ptr(Q), Q.shape[0], ptr(M), M.shape[0], Q.shape[1], int(device), ptr(approx), ptr(eps)))
+    return approx, eps

@@ -5,8 +5,9 @@
 // (:158-177), first index winning ties and only strictly positive scores counting (bestd
 // starts at 0, :150).  Here all questions are scored together as one Q x V x D contraction
 // on the tensor cores (w2b_eval_tc.cuh: TF32 wgmma fed by TMA, accumulators in registers) used as a FILTER
-// with a proven error bound, followed by an fp32 re-score of the surviving candidates in the reference's
-// operation order — so the arg-max is the reference's arg-max; the report text is the reference's, line for line.
+// with a proven error bound, followed by an fp32 re-score of the surviving candidates in the operation order of the
+// reference's build (gcc -O3 -march=x86-64-v3, oracle/Makefile) — so the arg-max is the reference's arg-max; the
+// report text is the reference's, line for line.
 #include <cuda_runtime.h>
 #include <ctype.h>
 #include <math.h>
@@ -52,7 +53,10 @@ struct FileCloser {
   ~FileCloser() { if (f && f != stdin) fclose(f); }
 };
 
-// quantize (:102) + L2 normalise (:103-106): one warp per row.
+// quantize (:106) + L2 normalise (:107-110): one warp per row.  len is summed in the order of the reference's build:
+// the squares of the first 4*floor(D/4) values are rounded on their own (vmulps) and added one at a time in index
+// order (vaddss); the last D mod 4 terms are fused (vfmadd231ss).  The lanes quantize and square 32 values at once;
+// every lane then adds the 32 in order (the same value in every lane, no reduction tree).
 __global__ void eval_normalize_kernel(float *M, long long words, long long D, long long Dp, int bits) {
   const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -61,14 +65,23 @@ __global__ void eval_normalize_kernel(float *M, long long words, long long D, lo
   qp.bits = bits;
   qp.seg = (bits >= 4) ? exp2f((float)(bits - 1)) : 1.f;
   float *r = M + row * Dp;  // rows are padded to Dp floats (zeros) for the tensor-core pass
+  const long long D4 = D & ~3LL;
   float s = 0.f;
-  for (long long a = lane; a < D; a += 32) {
-    const float q = quant<9>(r[a], qp);
-    r[a] = q;
-    s = fmaf(q, q, s);
+  for (long long a0 = 0; a0 < D; a0 += 32) {
+    const long long a = a0 + lane;
+    float q = 0.f;
+    if (a < D) {
+      q = quant<9>(r[a], qp);
+      r[a] = q;
+    }
+    const float p = __fmul_rn(q, q);
+    const int n = (int)min(32LL, D - a0);
+    for (int j = 0; j < n; ++j) {
+      const float pj = __shfl_sync(kFull, p, j), qj = __shfl_sync(kFull, q, j);
+      s = (a0 + j < D4) ? __fadd_rn(s, pj) : __fmaf_rn(qj, qj, s);
+    }
   }
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(kFull, s, o);
-  const float len = sqrtf(s);
+  const float len = __fsqrt_rn(s);
   for (long long a = lane; a < D; a += 32) r[a] = __fdiv_rn(r[a], len);
 }
 
@@ -81,9 +94,17 @@ __global__ void eval_query_kernel(const float *M, const int *q3, float *Q, long 
   Q[q * Dp + a] = __fadd_rn(__fsub_rn(M[b2 * Dp + a], M[b1 * Dp + a]), M[b3 * Dp + a]);
 }
 
-// eps of the tensor-core filter per question: TF32 keeps 10 explicit mantissa bits of each operand (the rest is
-// dropped), so each product is off by at most 2^-9 relative; with Cauchy-Schwarz |approx - exact| <= 2^-9 |vec| |m|,
-// |m| = 1 after normalisation; fp32 accumulation order (tensor core vs sequential) adds < 1e-4 |vec|.  5 % slack.
+// eps of the tensor-core filter per question, a bound on |approx - ref| where ref is the score in the reference's fp32
+// order and approx the tensor core's.  With u = 2^-24 and sum|v_a m_a| <= |vec| |m| (Cauchy-Schwarz), |m| = 1:
+//   operands: TF32 keeps 10 explicit mantissa bits of each (the rest is dropped), so a product is off by at most
+//             (1 + 2^-10)^2 - 1 < 2^-9 (1 + 2^-11) relative:                    <= 2^-9 (1 + 2^-11) |vec|
+//   tensor-core sum of Dp products: its fp32 accumulation is not specified; taken as truncating (unit 2u), Dp adds:
+//                                                                               <= 2 Dp u |vec| (1 + O(Dp u))
+//   reference sum: each product rounded once, then D rounded adds:              <= (D + 1) u |vec| (1 + O(D u))
+//   |m| and the |vec| computed here in fp32 are each within (D + 2) u of the true lengths; covered by one more
+//   Dp u term, and the (1 + O(Dp u)) factors by the 5 % slack for Dp u < 1/100 (Dp < 1.6e5; the reference's own
+//   limit is D <= 2000):
+//   eps = 1.05 |vec| (2^-9 (1 + 2^-11) + (4 Dp + 1) u).  At D = 800 the sum terms are 1.7e-4, at D = 2000 4.9e-4.
 __global__ void eval_qeps_kernel(const float *Q, float *qeps, long long nq, long long Dp) {
   const long long q = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
@@ -94,13 +115,13 @@ __global__ void eval_qeps_kernel(const float *Q, float *qeps, long long nq, long
     n2 = fmaf(x, x, n2);
   }
   for (int o = 16; o > 0; o >>= 1) n2 += __shfl_xor_sync(kFull, n2, o);
-  if (lane == 0) qeps[q] = (0.001953125f + 1e-4f) * 1.05f * sqrtf(n2);
+  if (lane == 0) qeps[q] = (0.001953125f * (1.f + 0x1p-11f) + (4.f * (float)Dp + 1.f) * 0x1p-24f) * 1.05f * sqrtf(n2);
 }
 
 // Pass 2: exact scores of the surviving candidates.  Thread per candidate: one whose approximate score is still
-// within 2*eps of the question's FINAL best is scored in fp32 exactly like the reference loop (:160-163) — dist = sum
-// over a ascending of vec[a] * M[a + c*size], one fused multiply-add per term, the order the fp32 SIMT scorer uses —
-// and competes for best[q] with the reference's rule: strictly positive, larger score wins, smaller index on ties.
+// within 2*eps of the question's FINAL best is scored in fp32 exactly like the reference's build runs :162-165 —
+// dist = sum over a ascending of vec[a] * M[a + c*size], each product rounded, then added (vmulss, vaddss: never
+// fused), the order the fp32 SIMT scorer uses — and competes for best[q] with the reference's rule: strictly positive, larger score wins, smaller index on ties.
 __global__ void eval_rescore_kernel(const float *Q, const float *M, const tc::Candidate *cand, unsigned long long n_cand,
                                     const float *qeps, const unsigned *gmax, unsigned long long *best,
                                     unsigned long long *n_rescored, int D, long long Dp) {
@@ -111,7 +132,7 @@ __global__ void eval_rescore_kernel(const float *Q, const float *M, const tc::Ca
   if (!(cd.s >= __uint_as_float(g & 0x7fffffffu) - 2.f * qeps[cd.q])) return;
   const float *v = Q + (size_t)cd.q * Dp, *m = M + (size_t)cd.c * Dp;
   float acc = 0.f;
-  for (int a = 0; a < D; ++a) acc = fmaf(v[a], m[a], acc);
+  for (int a = 0; a < D; ++a) acc = __fadd_rn(acc, __fmul_rn(v[a], m[a]));
   atomicAdd(n_rescored, 1ull);
   if (acc > 0.f)
     atomicMax(best + cd.q, ((unsigned long long)__float_as_uint(acc) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)cd.c));
@@ -156,7 +177,7 @@ __global__ void __launch_bounds__(256) eval_score_kernel(const float *Q, const f
 #pragma unroll
       for (int i = 0; i < 4; ++i)
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+        for (int j = 0; j < 4; ++j) acc[i][j] = __fadd_rn(acc[i][j], __fmul_rn(a[i], b[j]));
     }
     __syncthreads();
   }
@@ -231,26 +252,41 @@ static int read_vectors(const char *path, long long threshold, std::vector<std::
 
 static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t threshold,
                                  const char *questions_file, int device, w2b_accuracy *acc, char *report,
-                                 int64_t report_cap);
+                                 int64_t report_cap, int32_t *answers, int64_t answers_cap, int64_t *n_questions);
+// nothing is thrown across the C ABI (std::bad_alloc on a huge vocabulary, ...)
+template <class F> static int no_throw(const char *who, F &&f) {
+  try {
+    return f();
+  } catch (const std::exception &ex) {
+    w2b_set_error("%s: %s", who, ex.what());
+    return W2B_EINVAL;
+  } catch (...) {
+    w2b_set_error("%s: unexpected exception", who);
+    return W2B_EINVAL;
+  }
+}
 extern "C" int w2b_compute_accuracy(const char *vectors_file, int bitlevel, int64_t threshold,
                                     const char *questions_file, int device, w2b_accuracy *acc, char *report,
                                     int64_t report_cap) {
   if (!vectors_file) { w2b_set_error("w2b_compute_accuracy: null vectors_file"); return W2B_EINVAL; }
   if (report && report_cap > 0) report[0] = 0;
-  try {  // nothing is thrown across the C ABI (std::bad_alloc on a huge vocabulary, ...)
-    return compute_accuracy_impl(vectors_file, bitlevel, threshold, questions_file, device, acc, report, report_cap);
-  } catch (const std::exception &ex) {
-    w2b_set_error("w2b_compute_accuracy: %s", ex.what());
-    return W2B_EINVAL;
-  } catch (...) {
-    w2b_set_error("w2b_compute_accuracy: unexpected exception");
-    return W2B_EINVAL;
-  }
+  return no_throw("w2b_compute_accuracy", [&] {
+    return compute_accuracy_impl(vectors_file, bitlevel, threshold, questions_file, device, acc, report, report_cap,
+                                 nullptr, 0, nullptr);
+  });
+}
+extern "C" int w2b_analogy_answers(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file,
+                                   int device, int32_t *answers, int64_t answers_cap, int64_t *n_questions) {
+  if (!vectors_file) { w2b_set_error("w2b_analogy_answers: null vectors_file"); return W2B_EINVAL; }
+  return no_throw("w2b_analogy_answers", [&] {
+    return compute_accuracy_impl(vectors_file, bitlevel, threshold, questions_file, device, nullptr, nullptr, 0, answers,
+                                 answers_cap, n_questions);
+  });
 }
 
 static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t threshold,
                                  const char *questions_file, int device, w2b_accuracy *acc, char *report,
-                                 int64_t report_cap) {
+                                 int64_t report_cap, int32_t *answers, int64_t answers_cap, int64_t *n_questions) {
   std::vector<std::string> names;
   std::vector<float> M;
   long long words = 0, size = 0;
@@ -406,9 +442,10 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
       continue;
     }
     TQ++;
+    const unsigned long long key = e.qidx >= 0 ? best[e.qidx] : 0;
+    if (answers && TQ <= answers_cap) answers[TQ - 1] = key ? (int32_t)(0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull)) : -1;
     if (e.qidx < 0) continue;
     TQS++;
-    const unsigned long long key = best[e.qidx];
     std::string bestw;
     if (key) bestw = names[0xFFFFFFFFu - (unsigned)(key & 0xFFFFFFFFull)];
     if (e.st4 == bestw) {
@@ -421,6 +458,7 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
   }
   snprintf(line, sizeof line, "Questions seen / total: %d %d   %.2f %% \n", TQS, TQ, TQS / (float)TQ * 100);
   out += line;
+  if (n_questions) *n_questions = TQ;
   if (acc) {
     acc->questions_total = TQ; acc->questions_seen = TQS; acc->correct = CACN;
     acc->semantic_correct = SEAC; acc->semantic_seen = SECN; acc->syntactic_correct = SYAC; acc->syntactic_seen = SYCN;
@@ -431,4 +469,62 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
     report[report_cap - 1] = 0;
   }
   return W2B_OK;
+}
+
+// Test hook: the tensor-core filter's approximate score of every (question, word) pair and its eps per question.
+// Q (nq x D) and M (words x D) are used as given (no quantize, no normalisation: rows of M should have length <= 1
+// for eps to bound the error).  eval_tc_kernel runs unchanged, with eps = +inf (so every pair is a candidate), no
+// query words to skip and room for nq * words candidates; eps itself comes from eval_qeps_kernel.
+extern "C" int w2b_eval_filter_scores(const float *Q, int64_t nq, const float *M, int64_t words, int64_t D, int device,
+                                      float *approx, float *eps) {
+  if (!Q || !M || !approx || nq < 1 || words < 1 || D < 1 || nq * words > (1LL << 31)) {
+    w2b_set_error("w2b_eval_filter_scores: bad arguments");
+    return W2B_EINVAL;
+  }
+  return no_throw("w2b_eval_filter_scores", [&]() -> int {
+    CKE(cudaSetDevice(device));
+    const long long Dp = (D + tc::BK - 1) / tc::BK * tc::BK;
+    const unsigned long long cap = (unsigned long long)nq * (unsigned long long)words;
+    DevBuf bM, bQ, bq3, bgmax, bcand, bqeps, binf, bcnt;
+    CKE(bM.alloc((size_t)words * Dp * sizeof(float)));
+    CKE(bQ.alloc((size_t)nq * Dp * sizeof(float)));
+    CKE(bq3.alloc((size_t)nq * 3 * sizeof(int)));
+    CKE(bgmax.alloc(nq * sizeof(unsigned)));
+    CKE(bqeps.alloc(nq * sizeof(float)));
+    CKE(binf.alloc(nq * sizeof(float)));
+    CKE(bcnt.alloc(sizeof(unsigned long long)));
+    CKE(bcand.alloc(cap * sizeof(tc::Candidate)));
+    CKE(cudaMemset(bM.p, 0, (size_t)words * Dp * sizeof(float)));
+    CKE(cudaMemset(bQ.p, 0, (size_t)nq * Dp * sizeof(float)));
+    CKE(cudaMemcpy2D(bM.p, Dp * sizeof(float), M, D * sizeof(float), D * sizeof(float), words, cudaMemcpyHostToDevice));
+    CKE(cudaMemcpy2D(bQ.p, Dp * sizeof(float), Q, D * sizeof(float), D * sizeof(float), nq, cudaMemcpyHostToDevice));
+    CKE(cudaMemset(bq3.p, 0xff, (size_t)nq * 3 * sizeof(int)));  // -1: no query words
+    CKE(cudaMemset(bgmax.p, 0, nq * sizeof(unsigned)));
+    CKE(cudaMemset(bcnt.p, 0, sizeof(unsigned long long)));
+    std::vector<float> inf((size_t)nq, INFINITY);
+    CKE(cudaMemcpy(binf.p, inf.data(), nq * sizeof(float), cudaMemcpyHostToDevice));
+    CUtensorMap mapQ, mapM;
+    if (!tc::make_map(&mapQ, bQ.as<float>(), nq, Dp, tc::BM) || !tc::make_map(&mapM, bM.as<float>(), words, Dp, tc::BN)) {
+      w2b_set_error("cuTensorMapEncodeTiled failed (driver too old for TMA?)");
+      return W2B_ECUDA;
+    }
+    eval_qeps_kernel<<<(unsigned)((nq + 7) / 8), 256>>>(bQ.as<float>(), bqeps.as<float>(), nq, Dp);
+    CKE(cudaFuncSetAttribute(tc::eval_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
+    dim3 grid((unsigned)((nq + tc::BM - 1) / tc::BM), (unsigned)((words + tc::BN - 1) / tc::BN));
+    tc::eval_tc_kernel<<<grid, tc::THREADS, tc::SMEM_BYTES>>>(mapQ, mapM, bq3.as<int>(), binf.as<float>(), bgmax.as<unsigned>(),
+                                                             bcand.as<tc::Candidate>(), bcnt.as<unsigned long long>(), cap,
+                                                             (int)nq, (int)words, (int)Dp);
+    CKE(cudaGetLastError());
+    unsigned long long n = 0;
+    CKE(cudaMemcpy(&n, bcnt.p, sizeof n, cudaMemcpyDeviceToHost));
+    if (n != cap) {
+      w2b_set_error("w2b_eval_filter_scores: %llu of %llu pairs came through (NaN input?)", n, cap);
+      return W2B_EINVAL;
+    }
+    std::vector<tc::Candidate> cand((size_t)n);
+    CKE(cudaMemcpy(cand.data(), bcand.p, n * sizeof(tc::Candidate), cudaMemcpyDeviceToHost));
+    for (const tc::Candidate &c : cand) approx[(size_t)c.q * words + c.c] = c.s;
+    if (eps) CKE(cudaMemcpy(eps, bqeps.p, nq * sizeof(float), cudaMemcpyDeviceToHost));
+    return W2B_OK;
+  });
 }

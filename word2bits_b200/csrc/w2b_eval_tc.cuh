@@ -7,9 +7,11 @@
 //          4-stage mbarrier pipeline -> wgmma, accumulators in registers), 128 questions x 256 words per CTA;
 //          the epilogue keeps the question's best approximate score so far (atomicMax) and appends every
 //          (question, word) whose approximate score lies within 2*eps of the running best to a candidate list.  TF32 drops the low 13 mantissa bits of either operand, so
-//          |approx - exact| <= 2^-9 * |vec| * |m| (+ accumulation order): a bound, not a guess.
-//   pass 2 (w2b_eval.cu): candidates still within 2*eps of the FINAL best are re-scored in fp32 in the
-//          reference's operation order; the arg-max over them is the reference's arg-max.
+//          |approx - exact| <= 2^-9 * |vec| * |m| (+ the two fp32 accumulations, eval_qeps_kernel): a bound.
+//          A question with no positive approximate score keeps every word above -2*eps: the reference answers
+//          any word whose exact score is > 0.
+//   pass 2 (w2b_eval.cu): candidates still within 2*eps of the FINAL best (of 0 if none was positive) are
+//          re-scored in fp32 in the reference's operation order; the arg-max over them is the reference's arg-max.
 // Layout: both operands K-major with a row pitch of Dp = D rounded up to 32 floats (zero padding), so a k-block
 // is one 128-byte swizzle row; rows beyond nq / words are zero-filled by the TMA unit (OOB fill).
 #pragma once
@@ -170,7 +172,8 @@ eval_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
       for (int e = 0; e < 2; ++e) {
         const int c = n0 + 8 * j + 2 * (t & 3) + e;
         const float s = d[4 * j + 2 * h + e];
-        if (qok && c < words && c != b1 && c != b2 && c != b3 && s > 0.f && s >= thr) {
+        // s > -eps2, not s > 0: a word whose exact score is a little above 0 can have an approximate score <= 0
+        if (qok && c < words && c != b1 && c != b2 && c != b3 && s > -eps2 && s >= thr) {
           if (s > best) {
             best = s;
             thr = fmaxf(thr, s - eps2);  // (a superset is fine: thr only ever rises)
