@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "w2b.h"
@@ -103,17 +104,32 @@ static int nccl_load() {
 }
 enum { kNcclUint64 = 5, kNcclFloat32 = 7, kNcclSum = 0, kNcclAvg = 4 };
 
+// ------------------------------------------------------------------------------ plan
+typedef void (*train_fn)(TrainParams);
+typedef void (*apply_fn)(TrainParams, const int *, int, const int *, int, float *, double *);
+typedef void (*warp_fn)(TrainParams, int, int, ApplyArgs);
+
+// Which kernel trains a configuration and with what launch geometry (plan_config).
+struct Plan {
+  int rc = W2B_OK;      // validate(): W2B_EINVAL (message set) leaves the rest unplanned
+  long long pitch = 0;  // floats per row of u / v: layer1_size rounded up to a multiple of 4 (bulk copies move 16-byte units)
+  int vec = 4, ncol = 0, threads = 0;  // register kernel: floats per thread, threads with columns, threads per CTA
+  int group = 9;        // register kernel: target rows in flight per step (5, 9 or 13 are instantiated)
+  bool warp = false;    // production warp-per-shard kernel (csrc/w2b_warp.cuh) usable for this configuration
+  int warp_k = 0, warp_qcap = 0, warps_per_sm = 0;  // ring slots per warp, job queue entries, resident warps per SM
+  int warp_sen_smem = 1;  // the sentence buffer fits shared memory (else w2b_ctx::d_sen)
+  size_t warp_smem = 0;
+  warp_fn warp_kernel = nullptr;
+  train_fn train = nullptr;  // register kernel (configurations the warp kernel does not take)
+  apply_fn apply = nullptr;
+  size_t reg_smem = 0;       // register kernel's dynamic shared memory: strict mode keeps a row (D floats)
+};
+
 // ------------------------------------------------------------------------------ context
 struct w2b_ctx {
   w2b_config cfg;
   int nlocal = 0;  // shards owned by this context
-  long long pitch = 0;  // floats per row of u / v: layer1_size rounded up to a multiple of 4 (bulk copies move 16-byte units)
-  int vec = 4, ncol = 0, threads = 0, group = 9;
-  bool wide_train = false, wide_apply = false;  // register kernel: the 1024-thread (64-register) instantiations
-  bool warp = false;       // production warp-per-shard kernel (csrc/w2b_warp.cuh) usable for this configuration
-  int warp_k = 0, warp_qcap = 0, warp_minb = 0;  // ring slots per warp, job queue entries, warps per SM
-  int warp_sen_smem = 1;   // the sentence buffer fits shared memory (else d_sen)
-  size_t warp_smem = 0;
+  Plan plan;
   int *d_sen = nullptr;    // global sentence buffers: kMaxS ints per local shard (+ 1 for the parity hooks)
   int sm_count = 0;
   long long train_words = 0;
@@ -154,7 +170,7 @@ struct w2b_ctx {
 };
 
 static long long pitch_of(long long D) { return (D + 3) & ~3LL; }
-static size_t table_elems(const w2b_ctx *c) { return (size_t)c->cfg.vocab_size * (size_t)c->pitch; }
+static size_t table_elems(const w2b_ctx *c) { return (size_t)c->cfg.vocab_size * (size_t)c->plan.pitch; }
 
 static void lcg_tables(unsigned long long *JA, unsigned long long *JC, unsigned long long *PA,
                        unsigned long long *PC) {
@@ -173,177 +189,138 @@ static void lcg_tables(unsigned long long *JA, unsigned long long *JC, unsigned 
 }
 
 // ------------------------------------------------------------------------ kernel dispatch
-typedef void (*train_fn)(TrainParams);
-typedef void (*apply_fn)(TrainParams, const int *, int, const int *, int, float *, double *);
-
-template <int VEC, int BM, bool REG, bool STRICT, int G>
-static train_fn tk() { return train_shards_kernel<VEC, BM, REG, STRICT, G>; }
-template <int VEC, int BM, bool REG, bool STRICT, int G>
-static apply_fn ak() { return apply_position_kernel<VEC, BM, REG, STRICT, G>; }
-template <int VEC, bool REG, bool STRICT, int G>
-static train_fn tk_wide() { return train_shards_wide_kernel<VEC, 9, REG, STRICT, G>; }
-template <int VEC, bool REG, bool STRICT, int G>
-static apply_fn ak_wide() { return apply_position_wide_kernel<VEC, 9, REG, STRICT, G>; }
-
 static int bm_of(int bits) { return (bits == 0 || bits == 1 || bits == 2) ? bits : 9; }
 
-static train_fn pick_train(const w2b_ctx *c) {
-  const bool reg = c->cfg.reg != 0.f;
-  if (c->cfg.mode == W2B_MODE_STRICT) return c->vec == 4 ? tk_wide<4, true, true, 1>() : tk_wide<1, true, true, 1>();
-  if (c->wide_train) {
-    if (c->vec == 1) return reg ? tk_wide<1, true, false, 5>() : tk_wide<1, false, false, 5>();
-    return reg ? tk_wide<4, true, false, 5>() : tk_wide<4, false, false, 5>();
-  }
-  if (c->vec == 1) return reg ? tk<1, 9, true, false, 9>() : tk<1, 9, false, false, 9>();
-  const int bm = bm_of(c->cfg.bitlevel);
-#define W2B_PICK(BM)                                                         \
-  if (bm == BM) {                                                            \
-    if (reg) return tk<4, BM, true, false, 9>();                            \
-    if (c->group == 5) return tk<4, BM, false, false, 5>();                 \
-    if (c->group == 13) return tk<4, BM, false, false, 13>();               \
-    return tk<4, BM, false, false, 9>();                                    \
-  }
-  W2B_PICK(0) W2B_PICK(1) W2B_PICK(2) W2B_PICK(9)
-#undef W2B_PICK
-  return nullptr;
+// Strict mode, kernel = 1 and rows wider than 2048 floats run the register kernel; the warp kernel is not
+// instantiated beyond 2048.  validate() refuses the widths the register kernel cannot take by this predicate;
+// plan_config also sends a mode other than W2B_MODE_FAST (which validate() does not check) to the register kernel.
+static bool needs_register_kernel(const w2b_config &cfg) {
+  return cfg.mode == W2B_MODE_STRICT || cfg.kernel == 1 || cfg.layer1_size > 2048;
 }
 
-static apply_fn pick_apply(const w2b_ctx *c) {
-  const bool reg = c->cfg.reg != 0.f;
-  if (c->cfg.mode == W2B_MODE_STRICT) return c->vec == 4 ? ak_wide<4, true, true, 1>() : ak_wide<1, true, true, 1>();
-  if (c->wide_apply) {
-    if (c->vec == 1) return reg ? ak_wide<1, true, false, 5>() : ak_wide<1, false, false, 5>();
-    return reg ? ak_wide<4, true, false, 5>() : ak_wide<4, false, false, 5>();
+// ---- register kernel (csrc/w2b_kernels.cuh)
+struct RegKernel {
+  train_fn train;
+  apply_fn apply;
+};
+// Instantiations compiled for speed.  The apply hook runs G = 9 whatever the configuration's group.
+template <int VEC, int BM, bool REG, int G>
+static RegKernel reg_tuned() {
+  return {train_shards_kernel<VEC, BM, REG, false, G>, apply_position_kernel<VEC, BM, REG, false, 9>};
+}
+// __launch_bounds__(1024, 1) instantiations: bit level decided at run time, G = 5 (strict mode: 1).
+template <int VEC, bool REG, bool STRICT>
+static RegKernel reg_wide() {
+  constexpr int G = STRICT ? 1 : 5;
+  return {train_shards_wide_kernel<VEC, 9, REG, STRICT, G>, apply_position_wide_kernel<VEC, 9, REG, STRICT, G>};
+}
+template <int BM>
+static RegKernel reg_tuned_vec4(bool reg, int group) {
+  if (reg) return reg_tuned<4, BM, true, 9>();
+  if (group == 5) return reg_tuned<4, BM, false, 5>();
+  if (group == 13) return reg_tuned<4, BM, false, 13>();
+  return reg_tuned<4, BM, false, 9>();
+}
+// Strict mode always runs the wide instantiations; fast mode runs them when `wide` (plan_register_kernel), else the
+// speed-tuned ones, which compile the bit level in for VEC = 4 and run G = 9 with -reg or VEC = 1.
+static RegKernel register_kernel(const w2b_config &cfg, int vec, int group, bool wide) {
+  const bool reg = cfg.reg != 0.f;
+  if (cfg.mode == W2B_MODE_STRICT) return vec == 4 ? reg_wide<4, true, true>() : reg_wide<1, true, true>();
+  if (wide) {
+    if (vec == 1) return reg ? reg_wide<1, true, false>() : reg_wide<1, false, false>();
+    return reg ? reg_wide<4, true, false>() : reg_wide<4, false, false>();
   }
-  if (c->vec == 1) return reg ? ak<1, 9, true, false, 9>() : ak<1, 9, false, false, 9>();
-  const int bm = bm_of(c->cfg.bitlevel);
-#define W2B_PICK(BM)                                                         \
-  if (bm == BM) return reg ? ak<4, BM, true, false, 9>() : ak<4, BM, false, false, 9>();
-  W2B_PICK(0) W2B_PICK(1) W2B_PICK(2) W2B_PICK(9)
-#undef W2B_PICK
-  return nullptr;
+  if (vec == 1) return reg ? reg_tuned<1, 9, true, 9>() : reg_tuned<1, 9, false, 9>();
+  switch (bm_of(cfg.bitlevel)) {
+    case 0: return reg_tuned_vec4<0>(reg, group);
+    case 1: return reg_tuned_vec4<1>(reg, group);
+    case 2: return reg_tuned_vec4<2>(reg, group);
+    default: return reg_tuned_vec4<9>(reg, group);
+  }
 }
 
 // ---- warp-per-shard kernel (csrc/w2b_warp.cuh)
-typedef void (*warp_fn)(TrainParams, int, int, ApplyArgs);
-// warps (= 1-warp CTAs) per SM the register allocation is sized for; multiples of 4 because the register file is
-// split over the four SM sub-partitions: 12 warps -> 168 registers per thread, 16 -> 128, 20 -> 96, 24 -> 80.
-// Rows wider than 1024 floats (the reference publishes 1200-dimensional vectors): 8 warps (216 registers) up to
-// 1536 floats, 4 warps (248 registers) up to 2048.
-static int warp_minb_of(int nj) { return nj >= 13 ? 4 : (nj >= 9 ? 8 : (nj >= 5 ? 12 : (nj >= 3 ? 16 : (nj == 2 ? 20 : 24)))); }
-template <int BM>
-static warp_fn warp_by_nj(int nj) {
-  switch (nj) {
-    case 1: return train_warp_kernel<BM, 1, 24>;
-    case 2: return train_warp_kernel<BM, 2, 20>;
-    case 3: return train_warp_kernel<BM, 3, 16>;
-    case 4: return train_warp_kernel<BM, 4, 16>;
-    case 5: return train_warp_kernel<BM, 5, 12>;
-    case 6: return train_warp_kernel<BM, 6, 12>;
-    case 7: return train_warp_kernel<BM, 7, 12>;
-    case 8: return train_warp_kernel<BM, 8, 12>;
-    case 9: return train_warp_kernel<BM, 9, 8>;
-    case 10: return train_warp_kernel<BM, 10, 8>;
-    case 11: return train_warp_kernel<BM, 11, 8>;
-    case 12: return train_warp_kernel<BM, 12, 8>;
-    case 13: return train_warp_kernel<9, 13, 4>;  // (run-time bit level beyond 1536 floats: fewer instantiations)
-    case 14: return train_warp_kernel<9, 14, 4>;
-    case 15: return train_warp_kernel<9, 15, 4>;
-    case 16: return train_warp_kernel<9, 16, 4>;
-  }
-  return nullptr;
+// Warps (= 1-warp CTAs) per SM that train_warp_kernel<BM, NJ, MINB, REG> is compiled for (MINB) and plan_warp sizes
+// shared memory for.  Multiples of 4 because the register file is split over the four SM sub-partitions: 12 warps ->
+// 168 registers per thread, 16 -> 128, 20 -> 96, 24 -> 80.  Rows wider than 1024 floats (the reference publishes
+// 1200-dimensional vectors): 8 warps (216 registers) up to 1536 floats, 4 warps (248 registers) up to 2048.  -reg
+// keeps the raw row live: one step lower occupancy, at least 4 warps.
+static constexpr int warp_minb(int nj, bool reg) {
+  const int minb = nj >= 13 ? 4 : (nj >= 9 ? 8 : (nj >= 5 ? 12 : (nj >= 3 ? 16 : (nj == 2 ? 20 : 24))));
+  return reg ? std::max(4, minb - 4) : minb;
 }
-template <int NJ, int MINB>
-static warp_fn warp_reg() { return train_warp_kernel<9, NJ, MINB, 1>; }
-static warp_fn pick_warp(const w2b_ctx *c) {
-  const int nj = (int)((pitch_of(c->cfg.layer1_size) / 4 + 31) / 32);
-  if (c->cfg.reg != 0.f)  // -reg: one instantiation per width (run-time bit level; lower occupancy: the raw row stays live)
-    switch (nj) {
-      case 1: return warp_reg<1, 20>();
-      case 2: return warp_reg<2, 16>();
-      case 3: return warp_reg<3, 12>();
-      case 4: return warp_reg<4, 12>();
-      case 5: return warp_reg<5, 8>();
-      case 6: return warp_reg<6, 8>();
-      case 7: return warp_reg<7, 8>();
-      case 8: return warp_reg<8, 8>();
-      case 9: return warp_reg<9, 4>();
-      case 10: return warp_reg<10, 4>();
-      case 11: return warp_reg<11, 4>();
-      case 12: return warp_reg<12, 4>();
-      case 13: return warp_reg<13, 4>();
-      case 14: return warp_reg<14, 4>();
-      case 15: return warp_reg<15, 4>();
-      case 16: return warp_reg<16, 4>();
-    }
-  switch (bm_of(c->cfg.bitlevel)) {
-    case 0: return warp_by_nj<0>(nj);
-    case 1: return warp_by_nj<1>(nj);
-    case 2: return warp_by_nj<2>(nj);
-    default: return warp_by_nj<9>(nj);
+// Bit level compiled in (BM = 0, 1, 2) up to 1536 floats without -reg; decided at run time (BM = 9) beyond and with
+// -reg, for fewer instantiations.
+static constexpr int warp_bm(int bm, bool reg, int nj) { return reg || nj >= 13 ? 9 : bm; }
+// One instantiation per row width of NJ = I + 1 = 1 ... 16 column groups (32 float4s each).
+template <int BM, bool REG, int... I>
+static warp_fn warp_kernel_of(int nj, std::integer_sequence<int, I...>) {
+  static const warp_fn by_nj[] = {train_warp_kernel<warp_bm(BM, REG, I + 1), I + 1, warp_minb(I + 1, REG), REG>...};
+  return by_nj[nj - 1];
+}
+static warp_fn warp_kernel(const w2b_config &cfg, int nj) {
+  const auto widths = std::make_integer_sequence<int, 16>();
+  if (cfg.reg != 0.f) return warp_kernel_of<9, true>(nj, widths);
+  switch (bm_of(cfg.bitlevel)) {
+    case 0: return warp_kernel_of<0, false>(nj, widths);
+    case 1: return warp_kernel_of<1, false>(nj, widths);
+    case 2: return warp_kernel_of<2, false>(nj, widths);
+    default: return warp_kernel_of<9, false>(nj, widths);
   }
 }
+
 // Geometry: as many ring slots as the warp's share of the SM's 228 KB holds (each resident CTA also costs 1 KB of
 // reserved shared memory); at least 3 (one row being worked on, one draining, one in flight).
-static void plan_warp(w2b_ctx *c) {
-  c->warp = false;
-  if (c->cfg.mode != W2B_MODE_FAST || c->cfg.kernel == 1) return;
-  const long long pitch = pitch_of(c->cfg.layer1_size);
-  const int nj = (int)((pitch / 4 + 31) / 32);
-  if (nj > 16) return;  // kernels are instantiated for D <= 2048
-  const int minb = c->cfg.reg != 0.f ? (nj >= 9 ? 4 : (nj >= 5 ? 8 : (nj >= 3 ? 12 : (nj == 2 ? 16 : 20)))) : warp_minb_of(nj);
-  const int qcap = warp_queue_capacity(c->cfg.window, c->cfg.negative);
+static void plan_warp(const w2b_config &cfg, Plan *pl) {
+  const int nj = (int)((pl->pitch / 4 + 31) / 32);  // <= 16: D <= 2048
+  const int qcap = warp_queue_capacity(cfg.window, cfg.negative);
   // the sentence buffer (4000 B) moves to global memory when keeping it in shared memory would cost ring slots
   // below 4 (wide rows); a job queue too large for the warp's share of shared memory (very wide windows) is paid
   // for with fewer resident warps (the kernel compiled for `minb` warps runs at any lower occupancy)
-  int sen_smem = 1, K = 0, wps = minb;
+  int sen_smem = 1, K = 0, wps = warp_minb(nj, cfg.reg != 0.f);
   for (; wps >= 4; wps -= 4) {
     const size_t budget = (size_t)(228 * 1024) / wps - 1024;
     sen_smem = 1;
-    K = c->cfg.slots > 0 ? std::min(c->cfg.slots, 32) : 16;
-    while (K >= 3 && warp_layout(pitch, K, qcap, sen_smem).total > budget) --K;
+    K = cfg.slots > 0 ? std::min(cfg.slots, 32) : 16;
+    while (K >= 3 && warp_layout(pl->pitch, K, qcap, sen_smem).total > budget) --K;
     if (K < 4) {
-      int K2 = c->cfg.slots > 0 ? std::min(c->cfg.slots, 32) : 16;
-      while (K2 >= 3 && warp_layout(pitch, K2, qcap, 0).total > budget) --K2;
+      int K2 = cfg.slots > 0 ? std::min(cfg.slots, 32) : 16;
+      while (K2 >= 3 && warp_layout(pl->pitch, K2, qcap, 0).total > budget) --K2;
       if (K2 > K) { K = K2; sen_smem = 0; }
     }
     if (K >= 3) break;
   }
   if (wps < 4 || K < 3) return;
-  const int minb_eff = wps;
-  c->warp = true;
-  c->warp_k = K;
-  c->warp_qcap = qcap;
-  c->warp_minb = minb_eff;
-  c->warp_sen_smem = sen_smem;
-  c->warp_smem = warp_layout(pitch, K, qcap, sen_smem).total;
+  pl->warp = true;
+  pl->warp_k = K;
+  pl->warp_qcap = qcap;
+  pl->warps_per_sm = wps;
+  pl->warp_sen_smem = sen_smem;
+  pl->warp_smem = warp_layout(pl->pitch, K, qcap, sen_smem).total;
+  pl->warp_kernel = warp_kernel(cfg, nj);
 }
 
-// Register kernel (configurations the warp kernel does not take): c->threads threads per CTA.  The instantiations
+// Register kernel (configurations the warp kernel does not take): pl->threads threads per CTA.  The instantiations
 // compiled for speed run when they can take that many threads; otherwise the wide ones (__launch_bounds__(1024)).
 // A width that not even those can serve is refused here, at creation, instead of failing at its first launch.
-static int plan_register_kernel(w2b_ctx *c) {
-  c->wide_train = c->wide_apply = false;
+static int plan_register_kernel(const w2b_config &cfg, Plan *pl) {
+  const RegKernel wide = register_kernel(cfg, pl->vec, pl->group, true);
   cudaFuncAttributes fa;
-  if (c->cfg.mode != W2B_MODE_STRICT) {
-    CK(cudaFuncGetAttributes(&fa, (const void *)pick_train(c)));
-    c->wide_train = c->threads > fa.maxThreadsPerBlock;
-    CK(cudaFuncGetAttributes(&fa, (const void *)pick_apply(c)));
-    c->wide_apply = c->threads > fa.maxThreadsPerBlock;
+  if (cfg.mode != W2B_MODE_STRICT) {
+    CK(cudaFuncGetAttributes(&fa, (const void *)pl->train));
+    if (pl->threads > fa.maxThreadsPerBlock) pl->train = wide.train;
+    CK(cudaFuncGetAttributes(&fa, (const void *)pl->apply));
+    if (pl->threads > fa.maxThreadsPerBlock) pl->apply = wide.apply;
   }
-  for (const void *fn : {(const void *)pick_train(c), (const void *)pick_apply(c)}) {
+  for (const void *fn : {(const void *)pl->train, (const void *)pl->apply}) {
     CK(cudaFuncGetAttributes(&fa, fn));
-    if (c->threads > fa.maxThreadsPerBlock) {
+    if (pl->threads > fa.maxThreadsPerBlock) {
       w2b_set_error("layer1_size %lld needs %d threads per CTA; the register kernel takes at most %d for this "
-                    "configuration", (long long)c->cfg.layer1_size, c->threads, fa.maxThreadsPerBlock);
+                    "configuration", (long long)cfg.layer1_size, pl->threads, fa.maxThreadsPerBlock);
       return W2B_EINVAL;
     }
   }
   return W2B_OK;
-}
-
-static size_t dyn_smem(const w2b_ctx *c) {
-  return c->cfg.mode == W2B_MODE_STRICT ? (size_t)c->cfg.layer1_size * sizeof(float) : 0;
 }
 
 static TrainParams base_params(const w2b_ctx *c) {
@@ -359,9 +336,9 @@ static TrainParams base_params(const w2b_ctx *c) {
   p.alpha = c->d_alpha;
   p.wca = c->d_wca;
   p.D = c->cfg.layer1_size;
-  p.pitch = c->pitch;
+  p.pitch = c->plan.pitch;
   p.V = c->cfg.vocab_size;
-  p.ncol = c->ncol;
+  p.ncol = c->plan.ncol;
   p.window = c->cfg.window;
   p.negative = c->cfg.negative;
   p.bitlevel = c->cfg.bitlevel;
@@ -407,8 +384,7 @@ static int validate(const w2b_config *c) {
   // production kernel: any D <= 2048 (rows padded to whole float4s); register kernel: D <= 4096 when divisible by 4
   // (a thread per float4), else D <= 1024 (a thread per float) — strict mode and kernel = 1 always run the latter.
   // Every width accepted here launches (the wide instantiations, plan_register_kernel).
-  const bool reg_kernel = c->mode == W2B_MODE_STRICT || c->kernel == 1 || D > 2048;
-  if (D > 4096 || (reg_kernel && D % 4 != 0 && D > 1024)) {
+  if (D > 4096 || (needs_register_kernel(*c) && D % 4 != 0 && D > 1024)) {
     w2b_set_error("layer1_size %lld unsupported (at most 4096; in strict mode, with kernel 1 and above 2048 it must "
                   "also be divisible by 4 when above 1024)", D);
     return W2B_EINVAL;
@@ -416,32 +392,44 @@ static int validate(const w2b_config *c) {
   return W2B_OK;
 }
 
+// Everything the launches of a configuration depend on, without a CUDA call (w2b_warp_plan_query runs it on hosts
+// without a GPU).  The register kernel's instantiations are the speed-tuned ones in fast mode until
+// plan_register_kernel has checked them against the device.
+static Plan plan_config(const w2b_config &cfg) {
+  Plan pl;
+  pl.rc = validate(&cfg);
+  if (pl.rc) return pl;
+  const long long D = cfg.layer1_size;
+  pl.pitch = pitch_of(D);
+  pl.vec = (D % 4 == 0) ? 4 : 1;
+  pl.ncol = (int)((D + pl.vec - 1) / pl.vec);
+  pl.threads = std::max(32, (pl.ncol + 31) / 32 * 32);
+  pl.group = cfg.group ? cfg.group : (cfg.negative + 1 > 9 ? 13 : (cfg.negative + 1 > 5 ? 9 : 5));
+  if (pl.group != 5 && pl.group != 9 && pl.group != 13) pl.group = 9;  // register kernel instantiations
+  const RegKernel rk = register_kernel(cfg, pl.vec, pl.group, false);
+  pl.train = rk.train;
+  pl.apply = rk.apply;
+  pl.reg_smem = cfg.mode == W2B_MODE_STRICT ? (size_t)D * sizeof(float) : 0;
+  if (cfg.mode == W2B_MODE_FAST && !needs_register_kernel(cfg)) plan_warp(cfg, &pl);
+  return pl;
+}
+
 extern "C" int w2b_suggest_shards(const w2b_config *cfg, int *out) {
   NEED(cfg);
   NEED(out);
-  int rc = validate(cfg);
-  if (rc) return rc;
-  w2b_ctx tmp;
-  tmp.cfg = *cfg;
-  tmp.vec = (cfg->layer1_size % 4 == 0) ? 4 : 1;
-  tmp.ncol = (int)((cfg->layer1_size + tmp.vec - 1) / tmp.vec);
-  tmp.threads = std::max(32, (tmp.ncol + 31) / 32 * 32);
-  tmp.group = cfg->group ? cfg->group : (cfg->negative + 1 > 9 ? 13 : (cfg->negative + 1 > 5 ? 9 : 5));
+  Plan pl = plan_config(*cfg);
+  if (pl.rc) return pl.rc;
   CK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
   int per_sm = 0;
-  plan_warp(&tmp);
-  if (!tmp.warp) {
-    rc = plan_register_kernel(&tmp);
-    if (rc) return rc;
-  }
-  if (tmp.warp) {
-    warp_fn wf = pick_warp(&tmp);
-    CK(cudaFuncSetAttribute(wf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tmp.warp_smem));
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, wf, 32, tmp.warp_smem));
+  if (pl.warp) {
+    CK(cudaFuncSetAttribute(pl.warp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.warp_smem));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pl.warp_kernel, 32, pl.warp_smem));
   } else {
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pick_train(&tmp), tmp.threads, dyn_smem(&tmp)));
+    const int rc = plan_register_kernel(*cfg, &pl);
+    if (rc) return rc;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pl.train, pl.threads, pl.reg_smem));
   }
   *out = std::max(1, per_sm) * prop.multiProcessorCount;
   return W2B_OK;
@@ -450,21 +438,16 @@ extern "C" int w2b_suggest_shards(const w2b_config *cfg, int *out) {
 // ---- host-only views of the path's host logic (no CUDA call: usable, and tested, without a GPU)
 extern "C" int w2b_warp_plan_query(const w2b_config *cfg, w2b_warp_plan *out) {
   if (!cfg || !out) { w2b_set_error("null argument"); return W2B_EINVAL; }
-  int rc = validate(cfg);
-  if (rc) return rc;
-  w2b_ctx tmp;
-  tmp.cfg = *cfg;
-  tmp.vec = (cfg->layer1_size % 4 == 0) ? 4 : 1;
-  tmp.ncol = (int)((cfg->layer1_size + tmp.vec - 1) / tmp.vec);
-  plan_warp(&tmp);
+  const Plan pl = plan_config(*cfg);
+  if (pl.rc) return pl.rc;
   memset(out, 0, sizeof *out);
-  out->warp = tmp.warp ? 1 : 0;
-  if (!tmp.warp) return W2B_OK;
-  out->slots = tmp.warp_k;
-  out->sentence_in_smem = tmp.warp_sen_smem;
-  out->queue_entries = tmp.warp_qcap;
-  out->warps_per_sm = tmp.warp_minb;
-  out->smem_bytes = (int64_t)tmp.warp_smem;
+  out->warp = pl.warp ? 1 : 0;
+  if (!pl.warp) return W2B_OK;
+  out->slots = pl.warp_k;
+  out->sentence_in_smem = pl.warp_sen_smem;
+  out->queue_entries = pl.warp_qcap;
+  out->warps_per_sm = pl.warps_per_sm;
+  out->smem_bytes = (int64_t)pl.warp_smem;
   return W2B_OK;
 }
 
@@ -496,10 +479,10 @@ extern "C" int w2b_create(const w2b_config *cfg, w2b_ctx **out) {
 
 static int create_impl(const w2b_config *cfg, w2b_ctx **out) {
   *out = nullptr;
-  int rc = validate(cfg);
-  if (rc) return rc;
+  const Plan plan = plan_config(*cfg);
+  if (plan.rc) return plan.rc;
   int ndev = 0;
-  rc = w2b_device_count(&ndev);
+  int rc = w2b_device_count(&ndev);
   if (rc) return rc;
   if (ndev == 0 || cfg->device < 0 || cfg->device >= ndev) {
     w2b_set_error("no CUDA device %d (found %d): this library has no CPU fallback", cfg->device, ndev);
@@ -517,16 +500,10 @@ static int create_impl(const w2b_config *cfg, w2b_ctx **out) {
     return W2B_EINVAL;
   }
   c->nlocal = c->cfg.shard_end - c->cfg.shard_begin;
-  c->vec = (cfg->layer1_size % 4 == 0) ? 4 : 1;
-  c->ncol = (int)((cfg->layer1_size + c->vec - 1) / c->vec);
-  c->pitch = pitch_of(cfg->layer1_size);
-  c->threads = std::max(32, (c->ncol + 31) / 32 * 32);
-  c->group = cfg->group ? cfg->group : (cfg->negative + 1 > 9 ? 13 : (cfg->negative + 1 > 5 ? 9 : 5));
-  if (c->group != 5 && c->group != 9 && c->group != 13) c->group = 9;  // register kernel instantiations
-  plan_warp(c);
+  c->plan = plan;
   CK(cudaSetDevice(cfg->device));
-  if (!c->warp) {
-    rc = plan_register_kernel(c);
+  if (!c->plan.warp) {
+    rc = plan_register_kernel(*cfg, &c->plan);
     if (rc) return rc;
   }
   cudaDeviceProp prop;
@@ -546,7 +523,7 @@ static int create_impl(const w2b_config *cfg, w2b_ctx **out) {
   const size_t n = table_elems(c);
   CK(cudaMalloc(&c->d_u, n * sizeof(float)));
   CK(cudaMalloc(&c->d_v, n * sizeof(float)));
-  if (c->pitch != cfg->layer1_size) {  // padding columns start (and, in v, stay) at zero
+  if (c->plan.pitch != cfg->layer1_size) {  // padding columns start (and, in v, stay) at zero
     CK(cudaMemset(c->d_u, 0, n * sizeof(float)));
     CK(cudaMemset(c->d_v, 0, n * sizeof(float)));
   }
@@ -567,7 +544,7 @@ static int create_impl(const w2b_config *cfg, w2b_ctx **out) {
   }
   CK(cudaMalloc(&c->d_scratch, 64));
   CK(cudaMemset(c->d_scratch, 0, 64));
-  if (c->warp && !c->warp_sen_smem) CK(cudaMalloc(&c->d_sen, sizeof(int) * (size_t)kMaxS * (c->nlocal + 1)));
+  if (c->plan.warp && !c->plan.warp_sen_smem) CK(cudaMalloc(&c->d_sen, sizeof(int) * (size_t)kMaxS * (c->nlocal + 1)));
   CK(cudaEventCreate(&c->ev_s0));
   CK(cudaEventCreate(&c->ev_s1));
   // the memsets above ran on the legacy stream, which the context's non-blocking streams do not wait for
@@ -635,7 +612,7 @@ extern "C" int w2b_init_tables(w2b_ctx *c) {
   CK(cudaSetDevice(c->cfg.device));
   const long long n = c->cfg.vocab_size * c->cfg.layer1_size;
   const long long threads = (2 * n + 3) / 4;
-  init_net_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(c->d_v, c->d_u, n, c->cfg.layer1_size, c->pitch);
+  init_net_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, c->stream>>>(c->d_v, c->d_u, n, c->cfg.layer1_size, c->plan.pitch);
   CK(cudaGetLastError());
   float t[kExpN];
   w2b_exptable(t);
@@ -692,22 +669,25 @@ static int w2b_set_corpus_impl(w2b_ctx *c, const int32_t *ids, int64_t n, const 
   return w2b_epoch_begin(c);
 }
 
+// Local shard i's state at the start of an epoch.
+static ShardState shard_epoch_start(const w2b_ctx *c, int i) {
+  ShardState s;
+  memset(&s, 0, sizeof s);
+  s.rng = (unsigned long long)(long long)(c->cfg.shard_begin + i);  // :368
+  const bool ovr = c->shard_first[i] >= 0;
+  s.cursor = ovr ? c->shard_start[i] - 1 : c->shard_start[i];
+  s.ovr_idx = ovr ? c->shard_start[i] - 1 : -2;
+  s.ovr_tok = ovr ? c->shard_first[i] : -1;
+  s.limit = c->n_tokens;
+  s.limit_is_eof = 1;
+  return s;
+}
+
 extern "C" int w2b_epoch_begin(w2b_ctx *c) {
   NEED(c);
   if (!c->have_corpus) { w2b_set_error("set_corpus first"); return W2B_ESTATE; }
   CK(cudaSetDevice(c->cfg.device));
-  for (int i = 0; i < c->nlocal; ++i) {
-    ShardState &s = c->h_shards[i];
-    memset(&s, 0, sizeof s);
-    s.rng = (unsigned long long)(long long)(c->cfg.shard_begin + i);  // :368
-    const bool ovr = c->shard_first[i] >= 0;
-    s.cursor = ovr ? c->shard_start[i] - 1 : c->shard_start[i];
-    s.ovr_idx = ovr ? c->shard_start[i] - 1 : -2;
-    s.ovr_tok = ovr ? c->shard_first[i] : -1;
-    s.limit = c->n_tokens;
-    s.limit_is_eof = 1;
-    s.xlate = 0;
-  }
+  for (int i = 0; i < c->nlocal; ++i) c->h_shards[i] = shard_epoch_start(c, i);
   CK(cudaMemcpyAsync(c->d_shards, c->h_shards.data(), sizeof(ShardState) * c->nlocal, cudaMemcpyHostToDevice, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return W2B_OK;
@@ -821,34 +801,43 @@ static int stage_prefetch(w2b_ctx *c, long long chunk, w2b_step_stats *acc) {
   return W2B_OK;
 }
 
+// Launches the warp kernel: one warp (a 32-thread CTA) per local shard, or for a parity hook a single one that uses
+// the hooks' own sentence buffer, so that no shard's sentence is overwritten.
+static int launch_warp(const w2b_ctx *c, TrainParams p, const ApplyArgs &ap, bool hook) {
+  const Plan &pl = c->plan;
+  const warp_fn fn = pl.warp_kernel;
+  CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl.warp_smem));
+  if (hook && p.sen) p.sen += (size_t)kMaxS * c->nlocal;
+  fn<<<hook ? 1 : c->nlocal, 32, pl.warp_smem, c->stream>>>(p, pl.warp_k, pl.warp_qcap | (pl.warp_sen_smem << 31), ap);
+  return W2B_OK;
+}
+
+// Launches the register kernel's train or apply instantiation: `blocks` CTAs of plan.threads threads.
+template <class Fn, class... Args>
+static int launch_register(const w2b_ctx *c, Fn fn, int blocks, Args... args) {
+  const size_t smem = c->plan.reg_smem;
+  if (smem > 48 * 1024) CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  fn<<<blocks, c->plan.threads, smem, c->stream>>>(args...);
+  return W2B_OK;
+}
+
 // Enqueues the training kernel(s) of one launch on the context's stream (between ev0 and ev1).
 static int launch_enqueue(w2b_ctx *c, TrainParams p, w2b_step_stats *acc) {
   CK(cudaEventRecord(c->ev0, c->stream));
-  int launches = 1;
-  if (c->warp) {  // production path: one warp (a 32-thread CTA) per shard
-    warp_fn wf = pick_warp(c);
-    CK(cudaFuncSetAttribute(wf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->warp_smem));
-    p.shard_base = 0;
-    ApplyArgs none;
-    memset(&none, 0, sizeof none);
-    wf<<<c->nlocal, 32, c->warp_smem, c->stream>>>(p, c->warp_k, c->warp_qcap | (c->warp_sen_smem << 31), none);
-  } else {
-    train_fn fn = pick_train(c);
-    if (!fn) { w2b_set_error("no kernel for this configuration"); return W2B_EINVAL; }
-    const size_t smem = dyn_smem(c);
-    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (c->cfg.mode == W2B_MODE_STRICT) {
-      launches = 0;
-      for (int i = 0; i < c->nlocal; ++i) {  // shards one after another, like joined threads
-        p.shard_base = i;
-        fn<<<1, c->threads, smem, c->stream>>>(p);
-        ++launches;
-      }
-    } else {
-      p.shard_base = 0;
-      fn<<<c->nlocal, c->threads, smem, c->stream>>>(p);
+  int launches = 1, rc = W2B_OK;
+  if (c->plan.warp) {  // production path
+    rc = launch_warp(c, p, ApplyArgs{}, false);
+  } else if (c->cfg.mode == W2B_MODE_STRICT) {
+    launches = 0;
+    for (int i = 0; i < c->nlocal && !rc; ++i) {  // shards one after another, like joined threads
+      p.shard_base = i;
+      rc = launch_register(c, c->plan.train, 1, p);
+      ++launches;
     }
+  } else {
+    rc = launch_register(c, c->plan.train, c->nlocal, p);
   }
+  if (rc) return rc;
   CK(cudaGetLastError());
   CK(cudaEventRecord(c->ev1, c->stream));
   acc->launches += launches;
@@ -989,16 +978,7 @@ static int w2b_trace_impl(w2b_ctx *c, int shard, int64_t max_iterations, w2b_tra
   if (shard < c->cfg.shard_begin || shard >= c->cfg.shard_end) { w2b_set_error("shard not local"); return W2B_EINVAL; }
   CK(cudaSetDevice(c->cfg.device));
   // scratch copies: the draws must not disturb the training state
-  const int i = shard - c->cfg.shard_begin;
-  ShardState s;
-  memset(&s, 0, sizeof s);
-  s.rng = (unsigned long long)(long long)shard;
-  const bool ovr = c->shard_first[i] >= 0;
-  s.cursor = ovr ? c->shard_start[i] - 1 : c->shard_start[i];
-  s.ovr_idx = ovr ? c->shard_start[i] - 1 : -2;
-  s.ovr_tok = ovr ? c->shard_first[i] : -1;
-  s.limit = c->n_tokens;
-  s.limit_is_eof = 1;
+  const ShardState s = shard_epoch_start(c, shard - c->cfg.shard_begin);
   DevTmp t_s, t_alpha, t_cnt, t_tr;
   CK(t_s.alloc(sizeof s));
   CK(t_alpha.alloc(sizeof(float)));
@@ -1021,19 +1001,9 @@ static int w2b_trace_impl(w2b_ctx *c, int shard, int64_t max_iterations, w2b_tra
   p.train = 0;
   p.max_iters = max_iterations;
   p.wca_scale = 1;
-  if (c->warp) {  // the production kernel's own sampling code (prefetching draw path)
-    warp_fn wf = pick_warp(c);
-    CK(cudaFuncSetAttribute(wf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->warp_smem));
-    ApplyArgs none;
-    memset(&none, 0, sizeof none);
-    if (p.sen) p.sen += (size_t)kMaxS * c->nlocal;  // the hooks' own sentence buffer (block 0 of the launch)
-    wf<<<1, 32, c->warp_smem, c->stream>>>(p, c->warp_k, c->warp_qcap | (c->warp_sen_smem << 31), none);
-  } else {
-    train_fn fn = pick_train(c);
-    const size_t smem = dyn_smem(c);
-    if (smem > 48 * 1024) CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    fn<<<1, c->threads, smem, c->stream>>>(p);
-  }
+  // with the warp kernel: the production kernel's own sampling code (prefetching draw path)
+  const int rc = c->plan.warp ? launch_warp(c, p, ApplyArgs{}, true) : launch_register(c, c->plan.train, 1, p);
+  if (rc) return rc;
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(c->stream));
   unsigned long long cnt[2];
@@ -1057,11 +1027,9 @@ extern "C" int w2b_strict_prefix(w2b_ctx *c, int shard, int64_t max_iterations, 
   TrainParams p = base_params(c);
   p.shard_base = i;
   p.max_iters = max_iterations;
-  train_fn fn = pick_train(c);
-  const size_t smem = dyn_smem(c);
-  if (smem > 48 * 1024) CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const double before = c->h_shards[i].loss;
-  fn<<<1, c->threads, smem, c->stream>>>(p);
+  const int rc = launch_register(c, c->plan.train, 1, p);
+  if (rc) return rc;
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(c->h_shards.data(), c->d_shards, sizeof(ShardState) * c->nlocal, cudaMemcpyDeviceToHost,
                      c->stream));
@@ -1089,32 +1057,26 @@ extern "C" int w2b_apply_position(w2b_ctx *c, const int32_t *ctx_ids, int cw, co
   if (cw) CK(cudaMemcpyAsync(d_ids, ctx_ids, cw * sizeof(int), cudaMemcpyHostToDevice, c->stream));
   if (nt) CK(cudaMemcpyAsync(d_ids + cw, targets, nt * sizeof(int), cudaMemcpyHostToDevice, c->stream));
   TrainParams p = base_params(c);
-  if (c->warp) {  // L1 hook through the production kernel itself: one explicit position, one launch
+  if (c->plan.warp) {  // L1 hook through the production kernel itself: one explicit position, one launch
     if (cw > 2 * c->cfg.window || nt > c->cfg.negative + 1) {
       w2b_set_error("w2b_apply_position: cw <= 2*window and ntargets <= negative+1 for this context");
       return W2B_EINVAL;
     }
     if (cw == 0) return W2B_OK;  // nothing is trained without context (:450)
-    warp_fn wf = pick_warp(c);
-    CK(cudaFuncSetAttribute(wf, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->warp_smem));
     DevTmp t_s;
     CK(t_s.alloc(sizeof(ShardState)));
     CK(cudaMemsetAsync(t_s.p, 0, sizeof(ShardState), c->stream));
     p.shards = t_s.as<ShardState>();
     p.serial = 1;
-    ApplyArgs ap;
-    ap.ctx = d_ids; ap.tg = d_ids + cw; ap.cw = cw; ap.nt = nt; ap.f_out = d_f;
-    if (p.sen) p.sen += (size_t)kMaxS * c->nlocal;
-    wf<<<1, 32, c->warp_smem, c->stream>>>(p, c->warp_k, c->warp_qcap | (c->warp_sen_smem << 31), ap);
+    const int rc = launch_warp(c, p, ApplyArgs{d_ids, d_ids + cw, cw, nt, d_f}, true);
+    if (rc) return rc;
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(c->stream));
     if (f_out && nt) CK(cudaMemcpy(f_out, d_f, nt * sizeof(float), cudaMemcpyDeviceToHost));
     return W2B_OK;
   }
-  apply_fn fn = pick_apply(c);
-  const size_t smem = dyn_smem(c);
-  if (smem > 48 * 1024) CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  fn<<<1, c->threads, smem, c->stream>>>(p, d_ids, cw, d_ids + cw, nt, d_f, nullptr);
+  const int rc = launch_register(c, c->plan.apply, 1, p, d_ids, cw, d_ids + cw, nt, d_f, nullptr);
+  if (rc) return rc;
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(c->stream));
   if (f_out && nt) CK(cudaMemcpy(f_out, d_f, nt * sizeof(float), cudaMemcpyDeviceToHost));
@@ -1146,7 +1108,7 @@ extern "C" int w2b_set_state(w2b_ctx *c, float alpha, int64_t wca) {
 extern "C" int w2b_download_raw(w2b_ctx *c, float *u, float *v) {
   NEED(c);
   CK(cudaSetDevice(c->cfg.device));
-  const size_t row = (size_t)c->cfg.layer1_size * sizeof(float), dp = (size_t)c->pitch * sizeof(float);
+  const size_t row = (size_t)c->cfg.layer1_size * sizeof(float), dp = (size_t)c->plan.pitch * sizeof(float);
   if (u) CK(cudaMemcpy2D(u, row, c->d_u, dp, row, c->cfg.vocab_size, cudaMemcpyDeviceToHost));
   if (v) CK(cudaMemcpy2D(v, row, c->d_v, dp, row, c->cfg.vocab_size, cudaMemcpyDeviceToHost));
   return W2B_OK;
@@ -1155,7 +1117,7 @@ extern "C" int w2b_download_raw(w2b_ctx *c, float *u, float *v) {
 extern "C" int w2b_upload_raw(w2b_ctx *c, const float *u, const float *v) {
   NEED(c);
   CK(cudaSetDevice(c->cfg.device));
-  const size_t row = (size_t)c->cfg.layer1_size * sizeof(float), dp = (size_t)c->pitch * sizeof(float);
+  const size_t row = (size_t)c->cfg.layer1_size * sizeof(float), dp = (size_t)c->plan.pitch * sizeof(float);
   if (u) CK(cudaMemcpy2DAsync(c->d_u, dp, u, row, row, c->cfg.vocab_size, cudaMemcpyHostToDevice, c->stream));
   if (v) CK(cudaMemcpy2DAsync(c->d_v, dp, v, row, row, c->cfg.vocab_size, cudaMemcpyHostToDevice, c->stream));
   CK(cudaStreamSynchronize(c->stream));
@@ -1214,7 +1176,7 @@ static int w2b_checkpoint_save_impl(w2b_ctx *c, const char *path, int64_t epochs
   for (const float *src : {c->d_u, c->d_v})
     for (size_t r0 = 0; r0 < (size_t)h.V && ok; r0 += rows_per_piece) {
       const size_t nr = std::min(rows_per_piece, (size_t)h.V - r0);
-      if (cudaMemcpy2D(buf.data(), D * sizeof(float), src + r0 * c->pitch, (size_t)c->pitch * sizeof(float),
+      if (cudaMemcpy2D(buf.data(), D * sizeof(float), src + r0 * c->plan.pitch, (size_t)c->plan.pitch * sizeof(float),
                        D * sizeof(float), nr, cudaMemcpyDeviceToHost) != cudaSuccess) {
         fclose(f);
         remove(tmp.c_str());
@@ -1262,7 +1224,7 @@ static int w2b_checkpoint_load_impl(w2b_ctx *c, const char *path, int64_t *epoch
     for (size_t r0 = 0; r0 < (size_t)h.V; r0 += rows_per_piece) {
       const size_t nr = std::min(rows_per_piece, (size_t)h.V - r0);
       if (fread(buf.data(), sizeof(float), nr * D, f) != nr * D ||
-          cudaMemcpy2D(dst + r0 * c->pitch, (size_t)c->pitch * sizeof(float), buf.data(), D * sizeof(float),
+          cudaMemcpy2D(dst + r0 * c->plan.pitch, (size_t)c->plan.pitch * sizeof(float), buf.data(), D * sizeof(float),
                        D * sizeof(float), nr, cudaMemcpyHostToDevice) != cudaSuccess) {
         fclose(f);
         w2b_set_error("checkpoint %s is truncated or the upload failed", path);
@@ -1284,7 +1246,7 @@ extern "C" int w2b_export(w2b_ctx *c, float *out) {
   DevTmp t_out;
   CK(t_out.alloc(n * sizeof(float)));
   float *d_out = t_out.as<float>();
-  export_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->d_u, c->d_v, d_out, n, c->cfg.layer1_size, c->pitch, c->cfg.bitlevel);
+  export_kernel<<<c->sm_count * 8, 256, 0, c->stream>>>(c->d_u, c->d_v, d_out, n, c->cfg.layer1_size, c->plan.pitch, c->cfg.bitlevel);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, d_out, n * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
