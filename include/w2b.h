@@ -160,6 +160,25 @@ int w2b_suggest_shards(const w2b_config *cfg, int *out);
 int w2b_create(const w2b_config *cfg, w2b_ctx **out); /* globals :45-61 -> context */
 int w2b_destroy(w2b_ctx *ctx);
 
+/* The kernel instantiations a context launches: its training launches (w2b_train_step, w2b_train_epoch) and its
+ * single-position hook (w2b_apply_position).  Read-only. */
+typedef struct {
+  int32_t warp;        /* 1: train_warp_kernel<BM, NJ, MINB, REG> trains and serves the hook */
+  int32_t nj;          /* warp kernel: float4 column groups per lane */
+  int32_t minb;        /* warp kernel: resident warps per SM it is compiled for */
+  int32_t bm;          /* bit level compiled in (0, 1, 2), or 9 = decided at run time */
+  int32_t reg;         /* the -reg instantiation */
+  int32_t vec;         /* register kernel: floats per thread (4 or 1) */
+  int32_t threads;     /* register kernel: threads per CTA */
+  int32_t wide;        /* register kernel, training: 1 = train_shards_wide_kernel (__launch_bounds__(1024, 1)), 0 =
+                          the speed-tuned train_shards_kernel */
+  int32_t group;       /* register kernel, training: targets per group G (strict mode: 1 target at a time) */
+  int32_t apply_wide;  /* register kernel, hook: 1 = apply_position_wide_kernel, 0 = apply_position_kernel */
+  int32_t apply_bm;    /* register kernel, hook: bit level compiled in, or 9 */
+  int32_t apply_group; /* register kernel, hook: targets per group */
+} w2b_kernel_info;
+int w2b_kernel_query(w2b_ctx *ctx, w2b_kernel_info *out);
+
 /* vocab[].cn + train_words -> sub-sampling thresholds (:403-404) and the 1e8-entry
  * unigram table (InitUnigramTable, :112-128; boundaries on the host with the same libm
  * pow(), expanded on the device). */

@@ -179,6 +179,14 @@ class Trainer:
         check(lib.w2b_train_epoch(self.h, C.byref(loss), C.byref(st)))
         return loss.value, st.as_dict()
 
+    def kernel_info(self):
+        """The instantiations this context launches: {"warp": 1, "nj", "minb", "bm", "reg"} for the warp kernel; for the
+        register kernel vec, threads, bm, reg, and wide / group of the training launch and apply_* of the
+        single-position hook (w2b.h w2b_kernel_info)."""
+        out = _lib.KernelInfo()
+        check(lib.w2b_kernel_query(self.h, C.byref(out)))
+        return out.as_dict()
+
     # -- parity hooks
     def trace(self, shard, max_iterations=-1, cap=100000):
         recs = (_lib.TraceRec * cap)()

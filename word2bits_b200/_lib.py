@@ -54,6 +54,14 @@ class WarpPlan(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_}
 
 
+class KernelInfo(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("warp", "nj", "minb", "bm", "reg", "vec", "threads", "wide", "group",
+                                         "apply_wide", "apply_bm", "apply_group")]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
 class TraceRec(C.Structure):
     _fields_ = [("center", C.c_int32), ("b", C.c_int32), ("cw", C.c_int32), ("ntargets", C.c_int32),
                 ("targets", C.c_int32 * 64), ("alpha", C.c_float)]
@@ -71,6 +79,7 @@ EXPORTS = [
     "w2b_write_packed", "w2b_read_packed_header", "w2b_read_packed", "w2b_checkpoint_save", "w2b_checkpoint_load", "w2b_compute_accuracy",
     "w2b_analogy_answers", "w2b_eval_filter_scores",
     "w2b_host_unigram_bounds", "w2b_host_exptable", "w2b_host_keep_thresholds", "w2b_host_lcg_tables", "w2b_warp_plan_query", "w2b_host_gather_slices",
+    "w2b_kernel_query",
 ]
 
 if not os.path.exists(LIB_PATH):
@@ -115,6 +124,7 @@ lib.w2b_device_count.argtypes = [_P(C.c_int)]
 lib.w2b_suggest_shards.argtypes = [_P(Config), _P(C.c_int)]
 lib.w2b_create.argtypes = [_P(Config), _P(_vp)]
 lib.w2b_destroy.argtypes = [_vp]
+lib.w2b_kernel_query.argtypes = [_vp, _P(KernelInfo)]
 lib.w2b_set_vocab_counts.argtypes = [_vp, _vp, _i64, _i64]
 lib.w2b_set_corpus.argtypes = [_vp, _vp, _i64, _vp, _vp, C.c_int]
 lib.w2b_init_tables.argtypes = [_vp]

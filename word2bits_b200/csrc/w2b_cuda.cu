@@ -109,6 +109,16 @@ typedef void (*train_fn)(TrainParams);
 typedef void (*apply_fn)(TrainParams, const int *, int, const int *, int, float *, double *);
 typedef void (*warp_fn)(TrainParams, int, int, ApplyArgs);
 
+// Which register-kernel instantiation a train or apply pointer is (w2b_kernel_query).
+struct RegDesc {
+  int wide = 0;  // 1: the __launch_bounds__(1024, 1) copy
+  int vec = 0, bm = 0, reg = 0, group = 0;
+};
+// Which train_warp_kernel<BM, NJ, MINB, REG> instantiation a warp pointer is (w2b_kernel_query).
+struct WarpDesc {
+  int nj = 0, minb = 0, bm = 0, reg = 0;
+};
+
 // Which kernel trains a configuration and with what launch geometry (plan_config).
 struct Plan {
   int rc = W2B_OK;      // validate(): W2B_EINVAL (message set) leaves the rest unplanned
@@ -120,8 +130,10 @@ struct Plan {
   int warp_sen_smem = 1;  // the sentence buffer fits shared memory (else w2b_ctx::d_sen)
   size_t warp_smem = 0;
   warp_fn warp_kernel = nullptr;
+  WarpDesc warp_desc;
   train_fn train = nullptr;  // register kernel (configurations the warp kernel does not take)
   apply_fn apply = nullptr;
+  RegDesc train_desc, apply_desc;
   size_t reg_smem = 0;       // register kernel's dynamic shared memory: strict mode keeps a row (D floats)
 };
 
@@ -202,17 +214,20 @@ static bool needs_register_kernel(const w2b_config &cfg) {
 struct RegKernel {
   train_fn train;
   apply_fn apply;
+  RegDesc t, a;
 };
 // Instantiations compiled for speed.  The apply hook runs G = 9 whatever the configuration's group.
 template <int VEC, int BM, bool REG, int G>
 static RegKernel reg_tuned() {
-  return {train_shards_kernel<VEC, BM, REG, false, G>, apply_position_kernel<VEC, BM, REG, false, 9>};
+  return {train_shards_kernel<VEC, BM, REG, false, G>, apply_position_kernel<VEC, BM, REG, false, 9>,
+          {0, VEC, BM, REG, G}, {0, VEC, BM, REG, 9}};
 }
 // __launch_bounds__(1024, 1) instantiations: bit level decided at run time, G = 5 (strict mode: 1).
 template <int VEC, bool REG, bool STRICT>
 static RegKernel reg_wide() {
   constexpr int G = STRICT ? 1 : 5;
-  return {train_shards_wide_kernel<VEC, 9, REG, STRICT, G>, apply_position_wide_kernel<VEC, 9, REG, STRICT, G>};
+  return {train_shards_wide_kernel<VEC, 9, REG, STRICT, G>, apply_position_wide_kernel<VEC, 9, REG, STRICT, G>,
+          {1, VEC, 9, REG, G}, {1, VEC, 9, REG, G}};
 }
 template <int BM>
 static RegKernel reg_tuned_vec4(bool reg, int group) {
@@ -252,20 +267,22 @@ static constexpr int warp_minb(int nj, bool reg) {
 // Bit level compiled in (BM = 0, 1, 2) up to 1536 floats without -reg; decided at run time (BM = 9) beyond and with
 // -reg, for fewer instantiations.
 static constexpr int warp_bm(int bm, bool reg, int nj) { return reg || nj >= 13 ? 9 : bm; }
-// One instantiation per row width of NJ = I + 1 = 1 ... 16 column groups (32 float4s each).
+// One instantiation per row width of NJ = I + 1 = 1 ... 16 column groups (32 float4s each), with its descriptor.
 template <int BM, bool REG, int... I>
-static warp_fn warp_kernel_of(int nj, std::integer_sequence<int, I...>) {
+static warp_fn warp_kernel_of(int nj, std::integer_sequence<int, I...>, WarpDesc *desc) {
   static const warp_fn by_nj[] = {train_warp_kernel<warp_bm(BM, REG, I + 1), I + 1, warp_minb(I + 1, REG), REG>...};
+  static const WarpDesc descs[] = {{I + 1, warp_minb(I + 1, REG), warp_bm(BM, REG, I + 1), REG}...};
+  *desc = descs[nj - 1];
   return by_nj[nj - 1];
 }
-static warp_fn warp_kernel(const w2b_config &cfg, int nj) {
+static warp_fn warp_kernel(const w2b_config &cfg, int nj, WarpDesc *desc) {
   const auto widths = std::make_integer_sequence<int, 16>();
-  if (cfg.reg != 0.f) return warp_kernel_of<9, true>(nj, widths);
+  if (cfg.reg != 0.f) return warp_kernel_of<9, true>(nj, widths, desc);
   switch (bm_of(cfg.bitlevel)) {
-    case 0: return warp_kernel_of<0, false>(nj, widths);
-    case 1: return warp_kernel_of<1, false>(nj, widths);
-    case 2: return warp_kernel_of<2, false>(nj, widths);
-    default: return warp_kernel_of<9, false>(nj, widths);
+    case 0: return warp_kernel_of<0, false>(nj, widths, desc);
+    case 1: return warp_kernel_of<1, false>(nj, widths, desc);
+    case 2: return warp_kernel_of<2, false>(nj, widths, desc);
+    default: return warp_kernel_of<9, false>(nj, widths, desc);
   }
 }
 
@@ -297,7 +314,7 @@ static void plan_warp(const w2b_config &cfg, Plan *pl) {
   pl->warps_per_sm = wps;
   pl->warp_sen_smem = sen_smem;
   pl->warp_smem = warp_layout(pl->pitch, K, qcap, sen_smem).total;
-  pl->warp_kernel = warp_kernel(cfg, nj);
+  pl->warp_kernel = warp_kernel(cfg, nj, &pl->warp_desc);
 }
 
 // Register kernel (configurations the warp kernel does not take): pl->threads threads per CTA.  The instantiations
@@ -308,9 +325,9 @@ static int plan_register_kernel(const w2b_config &cfg, Plan *pl) {
   cudaFuncAttributes fa;
   if (cfg.mode != W2B_MODE_STRICT) {
     CK(cudaFuncGetAttributes(&fa, (const void *)pl->train));
-    if (pl->threads > fa.maxThreadsPerBlock) pl->train = wide.train;
+    if (pl->threads > fa.maxThreadsPerBlock) { pl->train = wide.train; pl->train_desc = wide.t; }
     CK(cudaFuncGetAttributes(&fa, (const void *)pl->apply));
-    if (pl->threads > fa.maxThreadsPerBlock) pl->apply = wide.apply;
+    if (pl->threads > fa.maxThreadsPerBlock) { pl->apply = wide.apply; pl->apply_desc = wide.a; }
   }
   for (const void *fn : {(const void *)pl->train, (const void *)pl->apply}) {
     CK(cudaFuncGetAttributes(&fa, fn));
@@ -409,6 +426,8 @@ static Plan plan_config(const w2b_config &cfg) {
   const RegKernel rk = register_kernel(cfg, pl.vec, pl.group, false);
   pl.train = rk.train;
   pl.apply = rk.apply;
+  pl.train_desc = rk.t;
+  pl.apply_desc = rk.a;
   pl.reg_smem = cfg.mode == W2B_MODE_STRICT ? (size_t)D * sizeof(float) : 0;
   if (cfg.mode == W2B_MODE_FAST && !needs_register_kernel(cfg)) plan_warp(cfg, &pl);
   return pl;
@@ -448,6 +467,31 @@ extern "C" int w2b_warp_plan_query(const w2b_config *cfg, w2b_warp_plan *out) {
   out->queue_entries = pl.warp_qcap;
   out->warps_per_sm = pl.warps_per_sm;
   out->smem_bytes = (int64_t)pl.warp_smem;
+  return W2B_OK;
+}
+
+extern "C" int w2b_kernel_query(w2b_ctx *c, w2b_kernel_info *out) {
+  NEED(c);
+  NEED(out);
+  const Plan &pl = c->plan;
+  memset(out, 0, sizeof *out);
+  if (pl.warp) {
+    out->warp = 1;
+    out->nj = pl.warp_desc.nj;
+    out->minb = pl.warp_desc.minb;
+    out->bm = pl.warp_desc.bm;
+    out->reg = pl.warp_desc.reg;
+    return W2B_OK;
+  }
+  out->threads = pl.threads;
+  out->vec = pl.train_desc.vec;
+  out->bm = pl.train_desc.bm;
+  out->reg = pl.train_desc.reg;
+  out->wide = pl.train_desc.wide;
+  out->group = pl.train_desc.group;
+  out->apply_wide = pl.apply_desc.wide;
+  out->apply_bm = pl.apply_desc.bm;
+  out->apply_group = pl.apply_desc.group;
   return W2B_OK;
 }
 
