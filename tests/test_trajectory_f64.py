@@ -47,7 +47,8 @@ LOG_1E9 = float(np.log(np.float32(1e-9)))
 def split_sentences(recs, W):
     """The draw trace cut into sentences: [(first record, number of records, kept-word ids)].  A sentence of L kept
     words has L records (one with center -1 when L = 0); its last record is the first whose cw has no right
-    neighbour (a = W + 1 is always inside the shrunk window because b < W)."""
+    neighbour (a = W + 1 is always inside the shrunk window because b < W).  A sentence the end of the trace cuts
+    off is left out."""
     out, i = [], 0
     while i < len(recs):
         if recs[i][0] < 0:
@@ -56,6 +57,8 @@ def split_sentences(recs, W):
             continue
         L = 1
         while True:
+            if i + L > len(recs):
+                return out
             b, cw = recs[i + L - 1][1], recs[i + L - 1][2]
             if cw == len([a for a in range(b, 2 * W + 1 - b) if a < W and L - 1 - W + a >= 0]):
                 break
@@ -200,6 +203,7 @@ class Replay:
         self.dup_taken = []  # warp kernel: 1 = a repeated target read its row after an earlier occurrence's update
         self.moved = True  # the last position changed something
         self.D = u0.shape[1]
+        self.hull = False  # take the hull of every admissible outcome instead of asking for a choice
 
     def copy(self, choices):
         c = object.__new__(Replay)
@@ -221,6 +225,10 @@ class Replay:
             T[i] = [src[i].astype(np.float64), np.zeros(self.D)]
         return T[i]
 
+    def read(self, T, src, i):
+        """Row i as a position reads it: [centre, radius] copies."""
+        return [x.copy() for x in self.row(T, src, i)]
+
     def quant(self, c, r):
         """Quantized values of the interval c +- r: the level, or where the interval holds two levels their hull."""
         if self.b == 0:
@@ -230,8 +238,9 @@ class Replay:
         self.straddles += int((ql != qh).sum())
         return (ql + qh) / 2, np.abs(qh - ql) / 2
 
-    def add_to(self, row, dc, dr):
-        """row += d as one rounded add (flushing denormal inputs and results)."""
+    def add_to(self, T, i, dc, dr):
+        """Row i of T += d as one rounded add (flushing denormal inputs and results)."""
+        row = T[i]
         row[0] = row[0] + dc
         row[1] = row[1] + dr + U * (np.abs(row[0]) + row[1]) + 2 * TINY
 
@@ -241,7 +250,7 @@ class Replay:
         d = float(np.float32(np.float32(2 * alpha) * self.reg))
         cw, nt = len(ctx), len(tg)
         # ---- context rows (:431-449)
-        pre = {i: [x.copy() for x in self.row(self.U, self.u0, i)] for i in set(ctx.tolist())}
+        pre = {i: self.read(self.U, self.u0, i) for i in set(ctx.tolist())}
         seen = {}
         qs_c, qs_r = np.zeros(D), np.zeros(D)
         s32, exact = np.zeros(D, np.float32), True  # every kernel sums the context rows in order, in float32
@@ -263,8 +272,7 @@ class Replay:
                 self.loss_c -= float(self.reg) * sq.sum()
                 self.loss_r += float(self.reg) * ((2 * np.abs(qc) * qr + qr * qr).sum() + gamma(D + 8) * (sq + 2 * np.abs(qc) * qr + qr * qr).sum())
             if m.kind == "warp" and d:  # the decay is scattered when the row is read
-                rowu = self.U[i]
-                self.add_to(rowu, -d * c, d * r + gamma(2) * d * (np.abs(c) + r))
+                self.add_to(self.U, i, -d * c, d * r + gamma(2) * d * (np.abs(c) + r))
         if exact:  # exact inputs: the float32 average itself (:449, IEEE division in every kernel)
             avg, r_avg = (s32 / np.float32(cw)).astype(np.float64), np.zeros(D)
         else:
@@ -279,22 +287,24 @@ class Replay:
         vpre = {}
         for t in range(nt):
             i = int(tg[t])
-            row = self.row(self.V, self.v0, i)
             if m.kind == "register" and t % m.G == 0:
-                snap = {k: [x.copy() for x in self.row(self.V, self.v0, int(k))] for k in tg[t:t + m.G]}
+                snap = {int(k): self.read(self.V, self.v0, int(k)) for k in tg[t:t + m.G]}
             if m.kind == "register":
                 xc, xr = snap[i]
             elif m.kind == "warp":
                 if i not in vpre:
-                    vpre[i] = [x.copy() for x in row]
+                    vpre[i] = self.read(self.V, self.v0, i)
                 xc, xr = vpre[i][0].copy(), vpre[i][1].copy()
                 for (_, dc, dr) in deltas.get(i, []):
+                    if self.hull:  # before or after the earlier occurrence's update
+                        xc, xr = xc + dc / 2, xr + np.abs(dc) / 2 + dr
+                        continue
                     self.dup_taken.append(self.choose(2))
                     if self.dup_taken[-1]:
                         xc += dc
                         xr = xr + dr
             else:
-                xc, xr = row[0].copy(), row[1].copy()
+                xc, xr = self.read(self.V, self.v0, i)
             qc, qr = self.quant(xc, xr)
             Q = np.abs(qc) + qr
             fc = float(avg @ qc)
@@ -303,7 +313,7 @@ class Replay:
             gs = g_candidates(fc, fr, label, alpha, self.ex)
             if len(gs) == 1:
                 gc, gr = gs[0], 0.0
-            elif len(gs) <= 3 and self.g_choices < 3:
+            elif not self.hull and len(gs) <= 3 and self.g_choices < 3:
                 self.g_choices += 1
                 gc, gr = gs[self.choose(len(gs))], 0.0
             else:  # f too uncertain, or too many such targets in the position to follow each: the hull of the values
@@ -328,17 +338,16 @@ class Replay:
             dr = abs(gc) * r_avg + gr * A + d * xr + gamma(3) * (G_ * A + d * X) + 3 * SUB
             if m.kind == "warp":
                 deltas.setdefault(i, []).append((t, dc, dr))
-            self.add_to(row, dc, dr)
+            self.add_to(self.V, i, dc, dr)
         e_r = e_r + gamma(nt + 1) * e_abs + nt * SUB
         # ---- the error to every context occurrence (:494-503)
         E = np.abs(e_c) + e_r
         for i in ctx.tolist():
-            rowu = self.U[i]
             if d and m.kind != "warp":  # decay of the row as this occurrence reads it
-                xc, xr = rowu[0].copy(), rowu[1].copy()
-                self.add_to(rowu, e_c - d * xc, e_r + d * xr + gamma(3) * (E + d * (np.abs(xc) + xr)) + 3 * SUB)
+                xc, xr = self.read(self.U, self.u0, i)
+                self.add_to(self.U, i, e_c - d * xc, e_r + d * xr + gamma(3) * (E + d * (np.abs(xc) + xr)) + 3 * SUB)
             else:
-                self.add_to(rowu, e_c, e_r)
+                self.add_to(self.U, i, e_c, e_r)
         self.moved = moved
 
     def final_rows_off(self, ids_u, ids_v, u1, v1):
@@ -366,7 +375,9 @@ def check_step(u0, v0, u1, v1, loss, positions, b, q, reg, exptab, model):
     """Checks one step.  Returns None when unresolved (more than MAX_BRANCHES admissible outcomes alive at once),
     else a dict of worst ratios (error / radius) of a branch that holds every element, or raises AssertionError naming
     the first failing element.  A branch is dropped as soon as a row whose last update in the step is done leaves its
-    interval, so a wrong expTable slot or a wrong before/after choice dies with its own target row."""
+    interval, so a wrong expTable slot or a wrong before/after choice dies with its own target row.  With loss None
+    only the rows the positions touch are compared, and the result carries the hull [loss_lo, loss_hi] of the
+    surviving branches' loss intervals."""
     last_u, last_v = {}, {}
     for p, (ctx, tg, _) in enumerate(positions):
         last_u.update((int(i), p) for i in ctx)
@@ -404,6 +415,7 @@ def check_step(u0, v0, u1, v1, loss, positions, b, q, reg, exptab, model):
     if not ok:
         raise AssertionError(min((r for r, _ in results), key=lambda r: r["worst"])["first"])
     res = ok[0][0]
+    res["loss_lo"], res["loss_hi"] = min(r["loss_lo"] for r, _ in ok), max(r["loss_hi"] for r, _ in ok)
     # the before (0) / after (1) reads every surviving branch agrees on: both were followed, so the other was rejected
     res["dups_forced"] = [x for x, *others in zip(*(d for _, d in ok)) if all(o == x for o in others)]
     return res
@@ -429,12 +441,18 @@ def compare(rp, u1, v1, loss):
             out["ok"] = False
             out["first"] = "%s row %d column %d: %r, replay %r +- %.3g" % (name, ids[k], col, after[ids[k], col],
                                                                         c[k, col], r[k, col])
+        if loss is None:
+            continue
         keep = np.ones(len(after), bool)
         keep[ids] = False
         if not np.array_equal(bits(after[keep]), bits(before[keep])):
             out["ok"] = False
             out["first"] = out["first"] or "%s: a row the step did not touch changed" % name
     lr = rp.loss_r + 1e-9 * abs(rp.loss_c)
+    out["loss_lo"], out["loss_hi"] = rp.loss_c - lr, rp.loss_c + lr
+    if loss is None:  # the replay's rows only; the caller checks the other rows and the loss
+        out["worst"] = max(out["u"], out["v"])
+        return out
     out["loss"] = abs(loss - rp.loss_c) / lr
     if out["loss"] > 1 and out["ok"]:
         out["ok"] = False
