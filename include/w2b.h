@@ -248,6 +248,23 @@ int w2b_analogy_answers(const char *vectors_file, int bitlevel, int64_t threshol
 int w2b_eval_filter_scores(const float *Q, int64_t nq, const float *M, int64_t words, int64_t D, int device,
                            float *approx, float *eps);
 
+/* The evaluator on a packed vector file (w2b_write_packed / -binary 2): same questions, same report text and the
+ * same chosen word per question as src/compute-accuracy.c gives on the unpacked file (w2b_read_packed ->
+ * w2b_write_vectors(binary=1)) with <bitlevel> = the file's bit level.  The table stays packed on the device: scores
+ * are exact integer dot products of bit planes (xor / popc), combined per question into a filter whose error bound
+ * covers fp32 rounding only, then the same fp32 re-score.  acc->candidates and acc->rescored count what they count
+ * above; acc->gpu_ms covers the plane, Gram, filter and re-score kernels. */
+int w2b_compute_accuracy_packed(const char *packed_file, int64_t threshold, const char *questions_file,
+                                int device, w2b_accuracy *acc, char *report, int64_t report_cap);
+int w2b_analogy_answers_packed(const char *packed_file, int64_t threshold, const char *questions_file,
+                               int device, int32_t *answers, int64_t answers_cap, int64_t *n_questions);
+/* Test hook: rows = V packed rows as in the file (ceil(D*bitlevel/8) bytes each, no names); for query word ids
+ * qid[0..W) gram[w*V + c] = the exact integer dot product of rows qid[w] and c in level units (1 bit: units of
+ * 1/9, 2 bits: 1/16); for questions q3[0..3*nq) (indices into qid) approx[q*V + c] = the filter's score and
+ * eps[q] the bound it uses on |approx - the reference's fp32 score|.  approx / eps may be NULL. */
+int w2b_eval_packed_scores(const uint8_t *rows, int64_t V, int64_t D, int bitlevel, const int32_t *qid, int64_t W,
+                           const int32_t *q3, int64_t nq, int device, int32_t *gram, float *approx, float *eps);
+
 /* Multi-GPU replica averaging (SURVEY §8(e)); G=1 contexts never touch NCCL. */
 int w2b_device_ptrs(w2b_ctx *ctx, void **u, void **v, int64_t *elems);
 int w2b_nccl_unique_id(void *id128);                                    /* ncclGetUniqueId */

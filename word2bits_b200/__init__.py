@@ -13,7 +13,8 @@ from . import _lib
 from ._lib import MODE_FAST, MODE_STRICT, TABLE_SIZE, W2BError, check, lib, ptr
 
 __all__ = ["Corpus", "Trainer", "W2BError", "MODE_FAST", "MODE_STRICT", "device_count", "read_packed", "nccl_unique_id",
-           "compute_accuracy", "analogy_answers", "eval_filter_scores", "host_unigram_bounds", "host_exptable", "host_keep_thresholds", "host_lcg_tables", "warp_plan"]
+           "compute_accuracy", "analogy_answers", "eval_filter_scores", "compute_accuracy_packed", "analogy_answers_packed",
+           "eval_packed_scores", "host_unigram_bounds", "host_exptable", "host_keep_thresholds", "host_lcg_tables", "warp_plan"]
 
 
 def device_count():
@@ -333,3 +334,40 @@ def eval_filter_scores(Q, M, device=0):
     eps = np.empty(Q.shape[0], np.float32)
     check(lib.w2b_eval_filter_scores(ptr(Q), Q.shape[0], ptr(M), M.shape[0], Q.shape[1], int(device), ptr(approx), ptr(eps)))
     return approx, eps
+
+
+def compute_accuracy_packed(packed_file, questions_file, threshold=0, device=0):
+    """compute_accuracy on a packed vector file (Corpus.write_packed / -binary 2), scored in the bit domain: returns
+    what compute_accuracy returns on the unpacked file with bitlevel = the file's bit level."""
+    acc = _lib.Accuracy()
+    buf = C.create_string_buffer(1 << 20)
+    check(lib.w2b_compute_accuracy_packed(packed_file.encode(), int(threshold), questions_file.encode(), int(device),
+                                          C.byref(acc), buf, len(buf)))
+    return buf.value.decode("latin1"), {k: getattr(acc, k) for k, _ in acc._fields_}
+
+
+def analogy_answers_packed(packed_file, questions_file, threshold=0, device=0):
+    """analogy_answers on a packed vector file."""
+    ans = np.empty(os.path.getsize(questions_file) // 4 + 1, np.int32)
+    n = C.c_int64()
+    check(lib.w2b_analogy_answers_packed(packed_file.encode(), int(threshold), questions_file.encode(), int(device),
+                                         ptr(ans), len(ans), C.byref(n)))
+    return ans[: n.value].copy()
+
+
+def eval_packed_scores(rows, D, bitlevel, qid, q3, device=0):
+    """Test hook of the packed evaluator: rows (V x ceil(D*bitlevel/8) uint8, packed as in the file), qid (W word
+    ids), q3 (nq x 3 indices into qid) -> (gram, approx, eps): gram[w, c] the exact integer dot product of rows qid[w]
+    and c in level units, approx[q, c] the filter's score, eps[q] its bound on |approx - the reference's score|."""
+    rows = np.ascontiguousarray(rows, np.uint8)
+    qid = np.ascontiguousarray(qid, np.int32)
+    q3 = np.ascontiguousarray(q3, np.int32).reshape(-1, 3)
+    V, W, nq = rows.shape[0], len(qid), len(q3)
+    if rows.shape[1] != (D * bitlevel + 7) // 8:
+        raise ValueError("rows must be ceil(D * bitlevel / 8) bytes wide")
+    gram = np.empty((W, V), np.int32)
+    approx = np.empty((nq, V), np.float32)
+    eps = np.empty(nq, np.float32)
+    check(lib.w2b_eval_packed_scores(ptr(rows), V, int(D), int(bitlevel), ptr(qid), W, ptr(q3), nq, int(device),
+                                     ptr(gram), ptr(approx), ptr(eps)))
+    return gram, approx, eps

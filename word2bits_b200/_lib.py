@@ -78,6 +78,7 @@ EXPORTS = [
     "w2b_device_ptrs", "w2b_nccl_unique_id", "w2b_nccl_init", "w2b_sync", "w2b_sync_timed", "w2b_table_checksum", "w2b_scale_tables",
     "w2b_write_packed", "w2b_read_packed_header", "w2b_read_packed", "w2b_checkpoint_save", "w2b_checkpoint_load", "w2b_compute_accuracy",
     "w2b_analogy_answers", "w2b_eval_filter_scores",
+    "w2b_compute_accuracy_packed", "w2b_analogy_answers_packed", "w2b_eval_packed_scores",
     "w2b_host_unigram_bounds", "w2b_host_exptable", "w2b_host_keep_thresholds", "w2b_host_lcg_tables", "w2b_warp_plan_query", "w2b_host_gather_slices",
     "w2b_kernel_query",
 ]
@@ -114,6 +115,9 @@ lib.w2b_checkpoint_load.argtypes = [_vp, C.c_char_p, _P(_i64)]
 lib.w2b_compute_accuracy.argtypes = [C.c_char_p, C.c_int, _i64, C.c_char_p, C.c_int, _P(Accuracy), C.c_char_p, _i64]
 lib.w2b_analogy_answers.argtypes = [C.c_char_p, C.c_int, _i64, C.c_char_p, C.c_int, _vp, _i64, _P(_i64)]
 lib.w2b_eval_filter_scores.argtypes = [_vp, _i64, _vp, _i64, _i64, C.c_int, _vp, _vp]
+lib.w2b_compute_accuracy_packed.argtypes = [C.c_char_p, _i64, C.c_char_p, C.c_int, _P(Accuracy), C.c_char_p, _i64]
+lib.w2b_analogy_answers_packed.argtypes = [C.c_char_p, _i64, C.c_char_p, C.c_int, _vp, _i64, _P(_i64)]
+lib.w2b_eval_packed_scores.argtypes = [_vp, _i64, _i64, C.c_int, _vp, _i64, _vp, _i64, C.c_int, _vp, _vp, _vp]
 lib.w2b_host_unigram_bounds.argtypes = [_vp, _i64, _vp]
 lib.w2b_host_exptable.argtypes = [_vp]
 lib.w2b_host_keep_thresholds.argtypes = [_vp, _i64, _i64, _f, _vp]

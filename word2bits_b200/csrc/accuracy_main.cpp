@@ -1,5 +1,7 @@
 // compute_accuracy — drop-in for the reference's evaluator (src/compute-accuracy.c), scored on the GPU.
 //   ./compute_accuracy <FILE> <bitlevel> <threshold> < questions-words.txt
+// FILE is a word2vec-binary vector file (first line "words size") or a packed one (`word2bits -binary 2`, first
+// line "words size bitlevel"), which is scored as it is, in the bit domain; <bitlevel> is then the file's or absent.
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -16,7 +18,19 @@ int main(int argc, char **argv) {
   const long long threshold = argc > 3 ? atoll(argv[3]) : 0;
   std::vector<char> report(1 << 20);
   w2b_accuracy acc;
-  const int rc = w2b_compute_accuracy(argv[1], bitlevel, threshold, nullptr, 0, &acc, report.data(), (long long)report.size());
+  long long words, size, packed_bits = 0;
+  char line[128], extra;
+  if (FILE *f = fopen(argv[1], "rb")) {  // three integers on the first line: a packed file
+    if (!fgets(line, sizeof line, f) || sscanf(line, "%lld %lld %lld %c", &words, &size, &packed_bits, &extra) != 3) packed_bits = 0;
+    fclose(f);
+  }
+  if (packed_bits && bitlevel != 0 && bitlevel != packed_bits) {
+    printf("%s holds %lld-bit vectors: <bitlevel> must be %lld, 0 or absent\n", argv[1], packed_bits, packed_bits);
+    return -1;
+  }
+  const int rc = packed_bits
+                     ? w2b_compute_accuracy_packed(argv[1], threshold, nullptr, 0, &acc, report.data(), (long long)report.size())
+                     : w2b_compute_accuracy(argv[1], bitlevel, threshold, nullptr, 0, &acc, report.data(), (long long)report.size());
   if (rc) {
     printf("%s\n", w2b_last_error());  // "Input file not found" (:83)
     return -1;

@@ -23,6 +23,7 @@
 #include "w2b_internal.h"
 #include "w2b_quant.cuh"
 #include "w2b_eval_tc.cuh"
+#include "w2b_eval_bits.cuh"
 
 using namespace w2b;
 
@@ -284,14 +285,17 @@ extern "C" int w2b_analogy_answers(const char *vectors_file, int bitlevel, int64
   });
 }
 
-static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t threshold,
-                                 const char *questions_file, int device, w2b_accuracy *acc, char *report,
-                                 int64_t report_cap, int32_t *answers, int64_t answers_cap, int64_t *n_questions) {
-  std::vector<std::string> names;
-  std::vector<float> M;
-  long long words = 0, size = 0;
-  int rc = read_vectors(vectors_file, threshold, names, M, words, size);
-  if (rc) return rc;
+// The question stream as the reference walks it: section headers and question lines in file order, and the three
+// query word ids of every question all of whose four words are in the vocabulary.
+struct Ev { int kind; std::string name; long long b1, b2, b3; std::string st4; int qidx; };  // 0 = section, 1 = question
+struct Questions {
+  std::vector<Ev> events;
+  std::vector<int> q3;
+};
+static int parse_questions(const char *questions_file, const std::vector<std::string> &names, Questions &qs) {
+  const long long words = (long long)names.size();
+  std::vector<Ev> &events = qs.events;
+  std::vector<int> &q3 = qs.q3;
   std::unordered_map<std::string, int> first;  // the reference's linear strcmp scan = first match (:140-145)
   for (long long b = words - 1; b >= 0; --b) first[names[b]] = (int)b;
   auto find = [&](const std::string &s) -> long long {
@@ -308,9 +312,6 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
     char buf[2048];
     while (fscanf(qf, "%2000s", buf) == 1) tok.push_back(buf);
   }
-  struct Ev { int kind; std::string name; long long b1, b2, b3; std::string st4; int qidx; };  // 0 = section, 1 = question
-  std::vector<Ev> events;
-  std::vector<int> q3;
   size_t t = 0;
   std::string st1;
   for (;;) {
@@ -335,6 +336,28 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
     }
     events.push_back(e);
   }
+  return W2B_OK;
+}
+
+// Replays the control flow of :113-187 over the chosen words (best[q] = score << 32 | ~index, 0 = none) to produce
+// the reference's report, the per-question answers and the counters.
+static void write_report(const Questions &qs, const std::vector<std::string> &names,
+                         const std::vector<unsigned long long> &best, long long words, long long size, float ms,
+                         w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers, int64_t answers_cap,
+                         int64_t *n_questions);
+
+static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t threshold,
+                                 const char *questions_file, int device, w2b_accuracy *acc, char *report,
+                                 int64_t report_cap, int32_t *answers, int64_t answers_cap, int64_t *n_questions) {
+  std::vector<std::string> names;
+  std::vector<float> M;
+  long long words = 0, size = 0;
+  int rc = read_vectors(vectors_file, threshold, names, M, words, size);
+  if (rc) return rc;
+  Questions qs;
+  rc = parse_questions(questions_file, names, qs);
+  if (rc) return rc;
+  const std::vector<int> &q3 = qs.q3;
   const long long nq = (long long)q3.size() / 3;
 
   // ---- GPU: normalise, build queries, tensor-core candidate pass, exact re-score of the candidate tiles
@@ -419,11 +442,18 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
     }
   }
 
-  // ---- replay the control flow of :113-187 to produce the same report
+  write_report(qs, names, best, words, size, ms, acc, report, report_cap, answers, answers_cap, n_questions);
+  return W2B_OK;
+}
+
+static void write_report(const Questions &qs, const std::vector<std::string> &names,
+                         const std::vector<unsigned long long> &best, long long words, long long size, float ms,
+                         w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers, int64_t answers_cap,
+                         int64_t *n_questions) {
   std::string out = "Starting eval...\n";
   char line[512];
   int TCN = 0, CCN = 0, TACN = 0, CACN = 0, SECN = 0, SYCN = 0, SEAC = 0, SYAC = 0, QID = 0, TQ = 0, TQS = 0;
-  for (const Ev &e : events) {
+  for (const Ev &e : qs.events) {
     if (e.kind == 0) {
       if (TCN == 0) TCN = 1;
       if (QID != 0) {
@@ -468,7 +498,6 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
     strncpy(report, out.c_str(), (size_t)report_cap - 1);
     report[report_cap - 1] = 0;
   }
-  return W2B_OK;
 }
 
 // Test hook: the tensor-core filter's approximate score of every (question, word) pair and its eps per question.
@@ -525,6 +554,289 @@ extern "C" int w2b_eval_filter_scores(const float *Q, int64_t nq, const float *M
     CKE(cudaMemcpy(cand.data(), bcand.p, n * sizeof(tc::Candidate), cudaMemcpyDeviceToHost));
     for (const tc::Candidate &c : cand) approx[(size_t)c.q * words + c.c] = c.s;
     if (eps) CKE(cudaMemcpy(eps, bqeps.p, nq * sizeof(float), cudaMemcpyDeviceToHost));
+    return W2B_OK;
+  });
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Packed vector files (w2b_write_packed / -binary 2): the table stays packed, scores are taken in the bit domain
+// (w2b_eval_bits.cuh).  The file format chooses this path; W2B_EVAL_SIMT=1, and a candidate list that overflows
+// (1-bit vectors at small D tie by the thousand), decode the planes to fp32 and run the fp32 SIMT scorer above.
+namespace {
+
+constexpr size_t kGramChunkBytes = 32u << 20;  // a chunk of G, written by the Gram kernel and read back by the filter
+
+struct HostPin {  // page-locks a host range for the duration of its copy
+  void *p = nullptr;
+  ~HostPin() { if (p) cudaHostUnregister(p); }
+};
+
+struct BitsState {
+  DevBuf rows, sign, mag, len, ilen, hpop, qid, q3, q3w, qk, qeps, gmax, cand, cnt, G;
+  long long V = 0, nbytes = 0, nq = 0, chunk = 0;
+  int D = 0, Wp = 0, W = 0;
+  unsigned long long cand_cap = 0;
+};
+
+// Device buffers of one run: rows = V packed rows nbytes apart, qid = the W distinct query words, q3w = per question
+// its three rows of G (indices into qid), q3 = per question the three vocabulary ids that cannot be its answer.
+int bits_upload(BitsState &st, const uint8_t *rows, long long V, int D, int bits, const int *qid, int W, const int *q3w,
+                const int *q3, long long nq, unsigned long long cand_cap) {
+  st.V = V; st.D = D; st.W = W; st.nq = nq; st.cand_cap = cand_cap;
+  st.nbytes = ((long long)D * bits + 7) / 8;
+  st.Wp = ((D + 31) / 32 + 3) & ~3;
+  const long long vround = (V + bits::CT - 1) / bits::CT * bits::CT;
+  st.chunk = std::min<long long>(vround, std::max<long long>(bits::CT, (long long)(kGramChunkBytes / 4 / W) / bits::CT * bits::CT));
+  CKE(st.rows.alloc((size_t)V * st.nbytes));
+  CKE(st.sign.alloc((size_t)V * st.Wp * 4));
+  if (bits == 2) CKE(st.mag.alloc((size_t)V * st.Wp * 4));
+  CKE(st.len.alloc(V * 4));
+  CKE(st.ilen.alloc(V * 4));
+  CKE(st.hpop.alloc(V * 4));
+  CKE(st.qid.alloc((size_t)W * 4));
+  CKE(st.q3.alloc((size_t)nq * 12));
+  CKE(st.q3w.alloc((size_t)nq * 12));
+  CKE(st.qk.alloc((size_t)nq * 12));
+  CKE(st.qeps.alloc((size_t)nq * 4));
+  CKE(st.gmax.alloc((size_t)nq * 4));
+  CKE(st.cnt.alloc(2 * sizeof(unsigned long long)));
+  CKE(st.cand.alloc(cand_cap * sizeof(tc::Candidate)));
+  CKE(st.G.alloc((size_t)W * st.chunk * 4));
+  HostPin pin;
+  CKE(cudaHostRegister((void *)rows, (size_t)V * st.nbytes, cudaHostRegisterDefault));
+  pin.p = (void *)rows;
+  CKE(cudaMemcpy(st.rows.p, rows, (size_t)V * st.nbytes, cudaMemcpyHostToDevice));
+  CKE(cudaMemcpy(st.qid.p, qid, (size_t)W * 4, cudaMemcpyHostToDevice));
+  CKE(cudaMemcpy(st.q3.p, q3, (size_t)nq * 12, cudaMemcpyHostToDevice));
+  CKE(cudaMemcpy(st.q3w.p, q3w, (size_t)nq * 12, cudaMemcpyHostToDevice));
+  CKE(cudaMemset(st.gmax.p, 0, (size_t)nq * 4));
+  CKE(cudaMemset(st.cnt.p, 0, 2 * sizeof(unsigned long long)));
+  return W2B_OK;
+}
+
+// planes + row lengths, then eps and the scale factors of every question
+template <int BITS> int bits_planes(BitsState &st) {
+  bits::eval_bits_planes_kernel<BITS><<<(unsigned)((st.V + 7) / 8), 256>>>(
+      st.rows.as<uint8_t>(), st.V, st.D, st.nbytes, st.Wp, st.sign.as<unsigned>(), st.mag.as<unsigned>(), st.len.as<float>(),
+      st.ilen.as<float>(), st.hpop.as<int>());
+  bits::eval_bits_qeps_kernel<BITS><<<(unsigned)((st.nq + 7) / 8), 256>>>(
+      st.sign.as<unsigned>(), st.mag.as<unsigned>(), st.len.as<float>(), st.qid.as<int>(), st.q3w.as<int>(), st.qk.as<float>(),
+      st.qeps.as<float>(), st.nq, st.D, st.Wp);
+  CKE(cudaGetLastError());
+  return W2B_OK;
+}
+
+// Gram + filter over the vocabulary, a chunk at a time; gram (host, W x V, may be NULL) receives every chunk of G.
+template <int BITS> int bits_filter(BitsState &st, int32_t *gram) {
+  for (long long c0 = 0; c0 < st.V; c0 += st.chunk) {
+    const int nc = (int)std::min(st.chunk, st.V - c0);
+    dim3 gg((unsigned)((nc + bits::GT - 1) / bits::GT), (unsigned)((st.W + bits::GT - 1) / bits::GT));
+    bits::eval_bits_gram_kernel<BITS><<<gg, 256>>>(st.sign.as<unsigned>(), st.mag.as<unsigned>(), st.hpop.as<int>(),
+                                                  st.qid.as<int>(), st.W, c0, nc, st.D, st.Wp, st.G.as<int>(), st.chunk);
+    // x = questions (fastest): every question meets the chunk's first tile before any meets its second
+    dim3 gc((unsigned)((st.nq + 7) / 8), (unsigned)((nc + bits::CT - 1) / bits::CT));
+    bits::eval_bits_combine_kernel<<<gc, 256>>>(st.G.as<int>(), st.chunk, c0, nc, st.ilen.as<float>(), st.q3.as<int>(),
+                                               st.q3w.as<int>(), st.qk.as<float>(), st.qeps.as<float>(), st.gmax.as<unsigned>(),
+                                               st.cand.as<tc::Candidate>(), st.cnt.as<unsigned long long>(), st.cand_cap,
+                                               (int)st.nq);
+    CKE(cudaGetLastError());
+    if (gram)
+      CKE(cudaMemcpy2D(gram + c0, (size_t)st.V * 4, st.G.p, (size_t)st.chunk * 4, (size_t)nc * 4, st.W, cudaMemcpyDeviceToHost));
+  }
+  return W2B_OK;
+}
+
+// Every score on the fp32 SIMT scorer: the planes become the fp32 table of the unpacked file, and
+// eval_normalize_kernel / eval_query_kernel / eval_score_kernel run as they do on a word2vec-binary file.
+template <int BITS> int bits_score_simt(BitsState &st, unsigned long long *dbest) {
+  const long long Dp = (st.D + tc::BK - 1) / tc::BK * tc::BK;
+  DevBuf bM, bQ;
+  CKE(bM.alloc((size_t)st.V * Dp * sizeof(float)));
+  CKE(bQ.alloc((size_t)st.nq * Dp * sizeof(float)));
+  CKE(cudaMemset(bM.p, 0, (size_t)st.V * Dp * sizeof(float)));
+  CKE(cudaMemset(bQ.p, 0, (size_t)st.nq * Dp * sizeof(float)));
+  CKE(cudaMemset(dbest, 0, st.nq * sizeof(unsigned long long)));
+  bits::eval_bits_decode_kernel<BITS><<<(unsigned)((st.V * st.D + 255) / 256), 256>>>(
+      st.sign.as<unsigned>(), st.mag.as<unsigned>(), bM.as<float>(), st.V, st.D, st.Wp, Dp);
+  eval_normalize_kernel<<<(unsigned)((st.V + 7) / 8), 256>>>(bM.as<float>(), st.V, st.D, Dp, BITS);
+  eval_query_kernel<<<(unsigned)((st.nq * st.D + 255) / 256), 256>>>(bM.as<float>(), st.q3.as<int>(), bQ.as<float>(), st.nq, st.D, Dp);
+  dim3 grid((unsigned)((st.V + TN - 1) / TN), (unsigned)((st.nq + TM - 1) / TM));
+  eval_score_kernel<<<grid, 256>>>(bQ.as<float>(), bM.as<float>(), st.q3.as<int>(), dbest, st.nq, st.V, st.D, Dp);
+  CKE(cudaGetLastError());
+  CKE(cudaDeviceSynchronize());  // bM and bQ are freed on return
+  return W2B_OK;
+}
+
+// best[q] of every question of a packed table; counts = {candidates, re-scored}
+template <int BITS> int bits_answers(BitsState &st, bool simt, unsigned long long *dbest, unsigned long long counts[2]) {
+  int rc = bits_planes<BITS>(st);
+  if (rc) return rc;
+  if (!simt) {
+    rc = bits_filter<BITS>(st, nullptr);
+    if (rc) return rc;
+    CKE(cudaMemcpy(counts, st.cnt.p, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    if (counts[0] > st.cand_cap) {
+      simt = true;
+    } else if (counts[0]) {
+      bits::eval_bits_rescore_kernel<BITS><<<(unsigned)((counts[0] + 127) / 128), 128>>>(
+          st.sign.as<unsigned>(), st.mag.as<unsigned>(), st.len.as<float>(), st.q3.as<int>(), st.cand.as<tc::Candidate>(),
+          counts[0], st.qeps.as<float>(), st.gmax.as<unsigned>(), dbest, st.cnt.as<unsigned long long>() + 1, st.D, st.Wp);
+      CKE(cudaGetLastError());
+    }
+  }
+  return simt ? bits_score_simt<BITS>(st, dbest) : W2B_OK;
+}
+
+int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, const char *questions_file, int device,
+                                 w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers,
+                                 int64_t answers_cap, int64_t *n_questions) {
+  w2b_packed_file pf;
+  int rc = w2b_packed_open(packed_file, &pf);
+  if (rc) return rc;
+  long long words = pf.V;
+  const long long size = pf.D;
+  if (threshold > 0 && words > threshold) words = threshold;
+  // D <= 2^17: the integer scores stay below 2^24 and eval_bits_qeps_kernel's slack holds
+  if (words < 1 || words > 0x7fffffffLL || size > (1LL << 17) || words > (1LL << 40) / pf.nbytes) {
+    w2b_set_error("bad header: %lld words of size %lld", words, size);
+    return W2B_EIO;
+  }
+  std::vector<std::string> names(words);
+  std::vector<uint8_t> rows((size_t)words * pf.nbytes);
+  for (long long b = 0; b < words; ++b) {
+    char raw[256];
+    rc = w2b_packed_next(&pf, raw, sizeof raw, &rows[(size_t)b * pf.nbytes]);
+    if (rc) return rc;
+    std::string w;  // read_vectors' rule for a name
+    for (const char *p = raw; *p; ++p)
+      if (*p != '\n' && w.size() < 50) w.push_back(*p);
+    names[b] = upper(w);
+  }
+  Questions qs;
+  rc = parse_questions(questions_file, names, qs);
+  if (rc) return rc;
+  const long long nq = (long long)qs.q3.size() / 3;
+  // the distinct query words: the Gram kernel runs once per word, not once per question
+  std::vector<int> qid, q3w(qs.q3.size());
+  {
+    std::unordered_map<int, int> row_of;
+    for (size_t i = 0; i < qs.q3.size(); ++i) {
+      auto it = row_of.emplace(qs.q3[i], (int)qid.size());
+      if (it.second) qid.push_back(qs.q3[i]);
+      q3w[i] = it.first->second;
+    }
+  }
+
+  std::vector<unsigned long long> best(nq > 0 ? nq : 1, 0);
+  float ms = 0.f;
+  if (nq > 0) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || device >= ndev) {
+      w2b_set_error("no CUDA device %d: the evaluator has no CPU fallback", device);
+      return W2B_ECUDA;
+    }
+    CKE(cudaSetDevice(device));
+    if (acc) acc->candidates = acc->rescored = 0;
+    const char *dbg = getenv("W2B_EVAL_SIMT");
+    const bool simt = dbg && atoi(dbg) != 0;
+    BitsState st;
+    DevBuf bbest;
+    rc = bits_upload(st, rows.data(), words, (int)size, pf.bits, qid.data(), (int)qid.size(), q3w.data(), qs.q3.data(), nq,
+                     (unsigned long long)nq * 1024ull);  // the cap of the tensor-core filter's list
+    if (rc) return rc;
+    CKE(bbest.alloc(nq * sizeof(unsigned long long)));
+    CKE(cudaMemset(bbest.p, 0, nq * sizeof(unsigned long long)));
+    DevEvent e0, e1;
+    CKE(cudaEventCreate(&e0.e));
+    CKE(cudaEventCreate(&e1.e));
+    CKE(cudaEventRecord(e0.e));
+    unsigned long long counts[2] = {0, 0};
+    rc = pf.bits == 1 ? bits_answers<1>(st, simt, bbest.as<unsigned long long>(), counts)
+                      : bits_answers<2>(st, simt, bbest.as<unsigned long long>(), counts);
+    if (rc) return rc;
+    CKE(cudaEventRecord(e1.e));
+    CKE(cudaMemcpy(best.data(), bbest.p, nq * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    CKE(cudaEventElapsedTime(&ms, e0.e, e1.e));
+    if (acc && !simt) {
+      CKE(cudaMemcpy(counts, st.cnt.p, sizeof(unsigned long long) * 2, cudaMemcpyDeviceToHost));
+      acc->candidates = (int64_t)counts[0];
+      acc->rescored = (int64_t)counts[1];
+    }
+  }
+  write_report(qs, names, best, words, size, ms, acc, report, report_cap, answers, answers_cap, n_questions);
+  return W2B_OK;
+}
+
+}  // namespace
+
+extern "C" int w2b_compute_accuracy_packed(const char *packed_file, int64_t threshold, const char *questions_file,
+                                           int device, w2b_accuracy *acc, char *report, int64_t report_cap) {
+  if (!packed_file) { w2b_set_error("w2b_compute_accuracy_packed: null packed_file"); return W2B_EINVAL; }
+  if (report && report_cap > 0) report[0] = 0;
+  return no_throw("w2b_compute_accuracy_packed", [&] {
+    return compute_accuracy_packed_impl(packed_file, threshold, questions_file, device, acc, report, report_cap, nullptr,
+                                        0, nullptr);
+  });
+}
+extern "C" int w2b_analogy_answers_packed(const char *packed_file, int64_t threshold, const char *questions_file,
+                                          int device, int32_t *answers, int64_t answers_cap, int64_t *n_questions) {
+  if (!packed_file || (!answers && answers_cap > 0)) {
+    w2b_set_error("w2b_analogy_answers_packed: null argument");
+    return W2B_EINVAL;
+  }
+  return no_throw("w2b_analogy_answers_packed", [&] {
+    return compute_accuracy_packed_impl(packed_file, threshold, questions_file, device, nullptr, nullptr, 0, answers,
+                                        answers_cap, n_questions);
+  });
+}
+
+// Test hook of the bit path: the Gram kernel's integers for explicit packed rows and query words, and the filter's
+// score of every (question, word) pair: eval_bits_combine_kernel runs unchanged with eps = +inf (every pair is a
+// candidate), no words to skip and room for nq * V candidates; eps itself comes from eval_bits_qeps_kernel.
+extern "C" int w2b_eval_packed_scores(const uint8_t *rows, int64_t V, int64_t D, int bitlevel, const int32_t *qid,
+                                      int64_t W, const int32_t *q3, int64_t nq, int device, int32_t *gram, float *approx,
+                                      float *eps) {
+  if (!rows || !qid || !gram || V < 1 || D < 1 || D > (1LL << 17) || (bitlevel != 1 && bitlevel != 2) || W < 1 || nq < 0 ||
+      (nq > 0 && !q3) || (approx && nq < 1) || W * V > (1LL << 31) || nq * V > (1LL << 31)) {
+    w2b_set_error("w2b_eval_packed_scores: bad arguments");
+    return W2B_EINVAL;
+  }
+  for (int64_t i = 0; i < W; ++i)
+    if (qid[i] < 0 || qid[i] >= V) { w2b_set_error("w2b_eval_packed_scores: qid[%lld] out of range", (long long)i); return W2B_EINVAL; }
+  for (int64_t i = 0; i < 3 * nq; ++i)
+    if (q3[i] < 0 || q3[i] >= W) { w2b_set_error("w2b_eval_packed_scores: q3[%lld] out of range", (long long)i); return W2B_EINVAL; }
+  return no_throw("w2b_eval_packed_scores", [&]() -> int {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || device >= ndev) {
+      w2b_set_error("no CUDA device %d: the evaluator has no CPU fallback", device);
+      return W2B_ECUDA;
+    }
+    CKE(cudaSetDevice(device));
+    const long long nqd = nq > 0 ? nq : 1;  // without questions: one that reads query word 0, its scores unused
+    std::vector<int> none((size_t)nqd * 3, -1), q3w((size_t)nqd * 3, 0);
+    if (nq > 0) q3w.assign(q3, q3 + 3 * nq);
+    const unsigned long long cap = approx ? (unsigned long long)nq * (unsigned long long)V : 1ull;
+    BitsState st;
+    int rc = bits_upload(st, rows, V, (int)D, bitlevel, qid, (int)W, q3w.data(), none.data(), nqd, cap);
+    if (rc) return rc;
+    rc = bitlevel == 1 ? bits_planes<1>(st) : bits_planes<2>(st);
+    if (rc) return rc;
+    if (eps && nq > 0) CKE(cudaMemcpy(eps, st.qeps.p, nq * sizeof(float), cudaMemcpyDeviceToHost));
+    std::vector<float> inf((size_t)nqd, INFINITY);
+    CKE(cudaMemcpy(st.qeps.p, inf.data(), nqd * sizeof(float), cudaMemcpyHostToDevice));
+    rc = bitlevel == 1 ? bits_filter<1>(st, gram) : bits_filter<2>(st, gram);
+    if (rc) return rc;
+    if (approx) {
+      unsigned long long n = 0;
+      CKE(cudaMemcpy(&n, st.cnt.p, sizeof n, cudaMemcpyDeviceToHost));
+      if (n != cap) {
+        w2b_set_error("w2b_eval_packed_scores: %llu of %llu pairs came through", n, cap);
+        return W2B_EINVAL;
+      }
+      std::vector<tc::Candidate> cand((size_t)n);
+      CKE(cudaMemcpy(cand.data(), st.cand.p, n * sizeof(tc::Candidate), cudaMemcpyDeviceToHost));
+      for (const tc::Candidate &c : cand) approx[(size_t)c.q * V + c.c] = c.s;
+    }
     return W2B_OK;
   });
 }

@@ -805,22 +805,46 @@ static int w2b_write_packed_impl(const char *path, const w2b_corpus *c, const fl
   return W2B_OK;
 }
 
-extern "C" int w2b_read_packed_header(const char *path, int64_t *V, int64_t *D, int *bitlevel) {
-  if (!path || !V || !D || !bitlevel) { w2b_set_error("w2b_read_packed_header: null argument"); return W2B_EINVAL; }
-  FILE *f = fopen(path, "rb");
-  if (!f) {
+int w2b_packed_open(const char *path, w2b_packed_file *pf) {
+  pf->f = fopen(path, "rb");
+  if (!pf->f) {
     w2b_set_error("cannot open %s", path);
     return W2B_EIO;
   }
-  long long v = 0, d = 0;
-  int b = 0;
-  const int n = fscanf(f, "%lld %lld %d", &v, &d, &b);
-  fclose(f);
-  if (n != 3 || (b != 1 && b != 2) || v < 0 || d < 1) {
+  char line[128];
+  long long v = 0, d = 0, b = 0;
+  char extra;
+  // three integers and nothing else on the first line: a word2vec-binary file has two
+  if (!fgets(line, sizeof line, pf->f) || !strchr(line, '\n') ||
+      sscanf(line, "%lld %lld %lld %c", &v, &d, &b, &extra) != 3 || (b != 1 && b != 2) || v < 0 || d < 1 ||
+      d > (INT64_MAX - 7) / 2) {
     w2b_set_error("%s is not a packed vector file", path);
     return W2B_EIO;
   }
-  *V = v; *D = d; *bitlevel = b;
+  pf->V = v; pf->D = d; pf->bits = (int)b;
+  pf->nbytes = (d * b + 7) / 8;
+  return W2B_OK;
+}
+
+int w2b_packed_next(w2b_packed_file *pf, char *name, int name_cap, uint8_t *row) {
+  int ch, k = 0;
+  while ((ch = fgetc(pf->f)) != EOF && ch != ' ')
+    if (name && k < name_cap - 1) name[k++] = (char)ch;
+  if (name) name[k] = 0;
+  if (fread(row, 1, pf->nbytes, pf->f) != (size_t)pf->nbytes) {
+    w2b_set_error("packed vector file is truncated");
+    return W2B_EIO;
+  }
+  fgetc(pf->f);  // '\n'
+  return W2B_OK;
+}
+
+extern "C" int w2b_read_packed_header(const char *path, int64_t *V, int64_t *D, int *bitlevel) {
+  if (!path || !V || !D || !bitlevel) { w2b_set_error("w2b_read_packed_header: null argument"); return W2B_EINVAL; }
+  w2b_packed_file pf;
+  const int rc = w2b_packed_open(path, &pf);
+  if (rc) return rc;
+  *V = pf.V; *D = pf.D; *bitlevel = pf.bits;
   return W2B_OK;
 }
 
@@ -830,35 +854,19 @@ extern "C" int w2b_read_packed(const char *path, float *vec, char *words, int ma
 }
 static int w2b_read_packed_impl(const char *path, float *vec, char *words, int max_word) {
   if (!path || !vec || (words && max_word < 1)) { w2b_set_error("w2b_read_packed: bad argument"); return W2B_EINVAL; }
-  int64_t V, D;
-  int bits;
-  int rc = w2b_read_packed_header(path, &V, &D, &bits);
+  w2b_packed_file pf;
+  int rc = w2b_packed_open(path, &pf);
   if (rc) return rc;
-  FILE *f = fopen(path, "rb");
-  if (!f) {
-    w2b_set_error("cannot open %s", path);
-    return W2B_EIO;
-  }
-  int ch;
-  while ((ch = fgetc(f)) != EOF && ch != '\n') {}
-  const int64_t nbytes = (D * bits + 7) / 8;
-  std::vector<uint8_t> row(nbytes);
-  for (int64_t a = 0; a < V; ++a) {
-    int k = 0;
-    while ((ch = fgetc(f)) != EOF && ch != ' ')
-      if (words && k < max_word - 1) words[a * max_word + k++] = (char)ch;
-    if (words) words[a * max_word + k] = 0;
-    if (fread(row.data(), 1, nbytes, f) != (size_t)nbytes) {
-      fclose(f);
-      w2b_set_error("%s is truncated", path);
-      return W2B_EIO;
-    }
+  const int64_t D = pf.D;
+  const int bits = pf.bits;
+  std::vector<uint8_t> row(pf.nbytes);
+  for (int64_t a = 0; a < pf.V; ++a) {
+    rc = w2b_packed_next(&pf, words ? words + a * max_word : nullptr, max_word, row.data());
+    if (rc) return rc;
     for (int64_t j = 0; j < D; ++j) {
       const int64_t bit = j * bits;
       vec[a * D + j] = level_value((row[bit >> 3] >> (bit & 7)) & ((1 << bits) - 1), bits);
     }
-    fgetc(f);  // '\n'
   }
-  fclose(f);
   return W2B_OK;
 }

@@ -1,6 +1,7 @@
 // Internal helpers shared by the host and device halves of libw2b (not part of the ABI).
 #pragma once
 #include <stdint.h>
+#include <stdio.h>
 
 #include <exception>
 #include <new>
@@ -24,6 +25,22 @@ static inline int w2b_guarded(const char *name, F &&body) {
     return 1;
   }
 }
+// The one parser of the packed vector format (w2b_write_packed): a header line "V D bitlevel", then per word its
+// name, ' ', nbytes = ceil(D * bitlevel / 8) bytes (value j in bits [j * bitlevel, (j + 1) * bitlevel), sign in the
+// low bit, for 2 bits the magnitude in the high bit) and '\n'.  w2b_read_packed expands rows to floats; the
+// evaluator keeps them packed.
+struct w2b_packed_file {
+  FILE *f = nullptr;
+  int64_t V = 0, D = 0, nbytes = 0;
+  int bits = 0;
+  ~w2b_packed_file() { if (f) fclose(f); }
+};
+// W2B_EIO unless the first line holds exactly three integers with V >= 0, D >= 1 and bitlevel 1 or 2; on success the
+// file is positioned at the first word.
+int w2b_packed_open(const char *path, w2b_packed_file *pf);
+// The next word: at most name_cap - 1 characters of its name (NUL-terminated; name may be NULL) and its nbytes
+// packed bytes.  W2B_EIO when the file ends inside the row.
+int w2b_packed_next(w2b_packed_file *pf, char *name, int name_cap, uint8_t *row);
 // InitUnigramTable (src/word2bits.cpp:112-128) in boundary form: start[i] = first table
 // slot owned by word i, start[V] = 1e8.  Same libm pow() and the same double arithmetic
 // as the reference loop, so expanding it reproduces the 1e8-entry table bit for bit.
