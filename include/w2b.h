@@ -265,6 +265,39 @@ int w2b_analogy_answers_packed(const char *packed_file, int64_t threshold, const
 int w2b_eval_packed_scores(const uint8_t *rows, int64_t V, int64_t D, int bitlevel, const int32_t *qid, int64_t W,
                            const int32_t *q3, int64_t nq, int device, int32_t *gram, float *approx, float *eps);
 
+/* Top-k lists: the reference's top-N list (src/compute-accuracy.c:166-175) at N = k, for analogy questions and for
+ * nearest neighbours.  A query is a question (b1, b2, b3), or a word w taken as the question (w, w, w), whose vec is
+ * M[w] exactly and which skips only w.  Its list holds the k largest fp32 scores > 0 (each product rounded, then
+ * added in index order, as the reference's build scores) of the words not in the query, in descending order, the
+ * smaller index first on equal scores; ids[i*k + j] = the word of rank j + 1 of the i-th query (-1 past the end of
+ * the list), scores[i*k + j] its score (0 with id -1).  A query with a word not in the vocabulary (only the first
+ * threshold words are searched, upper-cased, first match) gets an all -1 row.  1 <= k <= W2B_MAX_TOPK.
+ * Either file kind: a packed file (three integers on its first line) is scored in the bit domain, and bitlevel must
+ * then be 0 or the file's level.  The scores pass a TF32 or bit-domain filter that keeps every word within 2 eps of
+ * the query's running k-th best, then the survivors are scored exactly; a candidate list that overflows, and
+ * W2B_EVAL_SIMT=1, score every word exactly on the SIMT cores instead.  Queries run in batches that keep the
+ * candidate lists within 2 GB of device memory.  At most cap_queries rows are written; *n_queries = the number of
+ * queries; st (may be NULL) reports the run.  cap_queries = 0 only counts the queries (ids and scores may then be
+ * NULL; the vector file is not read). */
+#define W2B_MAX_TOPK 1024
+typedef struct {
+  float gpu_ms;              /* all kernels of the call, CUDA events (uploads of the table and the queries excluded) */
+  int64_t queries, skipped;  /* queries in the input; of which with a word not in the vocabulary */
+  int64_t chunks;            /* vocabulary chunks the filter ran over */
+  int64_t candidates;        /* (query, word) pairs the filter let through */
+  int64_t rescored;          /* ... of which within 2 eps of the final k-th best: scored exactly */
+  int32_t simt;              /* 1: the exact SIMT fall-back produced the lists (overflow or W2B_EVAL_SIMT=1) */
+  int32_t packed;            /* 1: the file was a packed (-binary 2) file, scored in the bit domain */
+} w2b_topk_stats;
+/* top-k lists of every question of questions_file (file order, as w2b_analogy_answers counts them; NULL = stdin) */
+int w2b_analogy_topk(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file, int k,
+                     int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries,
+                     w2b_topk_stats *st);
+/* nearest neighbours of every whitespace-separated word of words_file (NULL = stdin) */
+int w2b_nearest(const char *vectors_file, int bitlevel, int64_t threshold, const char *words_file, int k,
+                int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries,
+                w2b_topk_stats *st);
+
 /* Multi-GPU replica averaging (SURVEY §8(e)); G=1 contexts never touch NCCL. */
 int w2b_device_ptrs(w2b_ctx *ctx, void **u, void **v, int64_t *elems);
 int w2b_nccl_unique_id(void *id128);                                    /* ncclGetUniqueId */

@@ -14,7 +14,8 @@ from ._lib import MODE_FAST, MODE_STRICT, TABLE_SIZE, W2BError, check, lib, ptr
 
 __all__ = ["Corpus", "Trainer", "W2BError", "MODE_FAST", "MODE_STRICT", "device_count", "read_packed", "nccl_unique_id",
            "compute_accuracy", "analogy_answers", "eval_filter_scores", "compute_accuracy_packed", "analogy_answers_packed",
-           "eval_packed_scores", "host_unigram_bounds", "host_exptable", "host_keep_thresholds", "host_lcg_tables", "warp_plan"]
+           "eval_packed_scores", "host_unigram_bounds", "host_exptable", "host_keep_thresholds", "host_lcg_tables", "warp_plan",
+           "analogy_topk", "nearest"]
 
 
 def device_count():
@@ -371,3 +372,38 @@ def eval_packed_scores(rows, D, bitlevel, qid, q3, device=0):
     check(lib.w2b_eval_packed_scores(ptr(rows), V, int(D), int(bitlevel), ptr(qid), W, ptr(q3), nq, int(device),
                                      ptr(gram), ptr(approx), ptr(eps)))
     return gram, approx, eps
+
+
+def _topk(fn, vectors_file, input_file, k, bitlevel, threshold, device):
+    args = (vectors_file.encode(), int(bitlevel), int(threshold), input_file.encode() if input_file else None, int(k),
+            int(device))
+    n = C.c_int64()
+    check(fn(*args, None, None, 0, C.byref(n), None))  # counts the queries: the rows are sized exactly
+    ids = np.empty((max(n.value, 1), max(int(k), 1)), np.int32)
+    scores = np.empty(ids.shape, np.float32)
+    st = _lib.TopkStats()
+    check(fn(*args, ptr(ids), ptr(scores), max(n.value, 1), C.byref(n), C.byref(st)))
+    return ids[: n.value].copy(), scores[: n.value].copy(), st.as_dict()
+
+
+def analogy_topk(vectors_file, questions_file, k, bitlevel=0, threshold=0, device=0):
+    """The reference's top-N list at N = k for every question of questions_file, in file order: (ids int32 [n, k],
+    scores float32 [n, k], stats).  Row i holds the k words of largest fp32 score > 0 (not the question's own words),
+    best first, the smaller index first on equal scores; -1 (score 0) pads a short list and fills the row of a question
+    with a word not in the vocabulary.  Word2vec-binary or packed vector file (bitlevel then 0 or the file's)."""
+    return _topk(lib.w2b_analogy_topk, vectors_file, questions_file, k, bitlevel, threshold, device)
+
+
+def nearest(vectors_file, words, k, bitlevel=0, threshold=0, device=0):
+    """Nearest neighbours: the list of analogy_topk for the question (w, w, w) of every word w of `words` (a list of
+    words, or the path of a file of whitespace-separated words): the k words whose vectors have the largest cosine
+    with w's, w itself excluded.  Returns (ids int32 [n, k], scores float32 [n, k], stats)."""
+    if isinstance(words, (list, tuple)):
+        import tempfile
+        with tempfile.NamedTemporaryFile("w", suffix=".txt", delete=False) as f:
+            f.write("\n".join(words) + "\n")
+        try:
+            return _topk(lib.w2b_nearest, vectors_file, f.name, k, bitlevel, threshold, device)
+        finally:
+            os.unlink(f.name)
+    return _topk(lib.w2b_nearest, vectors_file, words, k, bitlevel, threshold, device)

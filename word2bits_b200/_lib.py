@@ -46,6 +46,17 @@ class Accuracy(C.Structure):
                [("gpu_ms", C.c_float), ("candidates", C.c_int64), ("rescored", C.c_int64)]
 
 
+class TopkStats(C.Structure):
+    _fields_ = [("gpu_ms", C.c_float), ("queries", C.c_int64), ("skipped", C.c_int64), ("chunks", C.c_int64),
+                ("candidates", C.c_int64), ("rescored", C.c_int64), ("simt", C.c_int32), ("packed", C.c_int32)]
+
+    def as_dict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+MAX_TOPK = 1024
+
+
 class WarpPlan(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("warp", "slots", "queue_entries", "warps_per_sm", "sentence_in_smem", "reserved")] + \
                [("smem_bytes", C.c_int64)]
@@ -79,6 +90,7 @@ EXPORTS = [
     "w2b_write_packed", "w2b_read_packed_header", "w2b_read_packed", "w2b_checkpoint_save", "w2b_checkpoint_load", "w2b_compute_accuracy",
     "w2b_analogy_answers", "w2b_eval_filter_scores",
     "w2b_compute_accuracy_packed", "w2b_analogy_answers_packed", "w2b_eval_packed_scores",
+    "w2b_analogy_topk", "w2b_nearest",
     "w2b_host_unigram_bounds", "w2b_host_exptable", "w2b_host_keep_thresholds", "w2b_host_lcg_tables", "w2b_warp_plan_query", "w2b_host_gather_slices",
     "w2b_kernel_query",
 ]
@@ -118,6 +130,10 @@ lib.w2b_eval_filter_scores.argtypes = [_vp, _i64, _vp, _i64, _i64, C.c_int, _vp,
 lib.w2b_compute_accuracy_packed.argtypes = [C.c_char_p, _i64, C.c_char_p, C.c_int, _P(Accuracy), C.c_char_p, _i64]
 lib.w2b_analogy_answers_packed.argtypes = [C.c_char_p, _i64, C.c_char_p, C.c_int, _vp, _i64, _P(_i64)]
 lib.w2b_eval_packed_scores.argtypes = [_vp, _i64, _i64, C.c_int, _vp, _i64, _vp, _i64, C.c_int, _vp, _vp, _vp]
+lib.w2b_analogy_topk.argtypes = [C.c_char_p, C.c_int, _i64, C.c_char_p, C.c_int, C.c_int, _vp, _vp, _i64, _P(_i64),
+                                 _P(TopkStats)]
+lib.w2b_nearest.argtypes = [C.c_char_p, C.c_int, _i64, C.c_char_p, C.c_int, C.c_int, _vp, _vp, _i64, _P(_i64),
+                            _P(TopkStats)]
 lib.w2b_host_unigram_bounds.argtypes = [_vp, _i64, _vp]
 lib.w2b_host_exptable.argtypes = [_vp]
 lib.w2b_host_keep_thresholds.argtypes = [_vp, _i64, _i64, _f, _vp]

@@ -24,6 +24,7 @@
 #include "w2b_quant.cuh"
 #include "w2b_eval_tc.cuh"
 #include "w2b_eval_bits.cuh"
+#include "w2b_eval_topk.cuh"
 
 using namespace w2b;
 
@@ -41,7 +42,11 @@ namespace {
 // device buffers / events released on every return path
 struct DevBuf {
   void *p = nullptr;
-  ~DevBuf() { if (p) cudaFree(p); }
+  ~DevBuf() { reset(); }
+  void reset() {
+    if (p) cudaFree(p);
+    p = nullptr;
+  }
   cudaError_t alloc(size_t bytes) { return cudaMalloc(&p, bytes ? bytes : 1); }
   template <class T> T *as() const { return static_cast<T *>(p); }
 };
@@ -131,9 +136,7 @@ __global__ void eval_rescore_kernel(const float *Q, const float *M, const tc::Ca
   const tc::Candidate cd = cand[i];
   const unsigned g = gmax[cd.q];
   if (!(cd.s >= __uint_as_float(g & 0x7fffffffu) - 2.f * qeps[cd.q])) return;
-  const float *v = Q + (size_t)cd.q * Dp, *m = M + (size_t)cd.c * Dp;
-  float acc = 0.f;
-  for (int a = 0; a < D; ++a) acc = __fadd_rn(acc, __fmul_rn(v[a], m[a]));
+  const float acc = fp32_score(Q + (size_t)cd.q * Dp, M + (size_t)cd.c * Dp, D);
   atomicAdd(n_rescored, 1ull);
   if (acc > 0.f)
     atomicMax(best + cd.q, ((unsigned long long)__float_as_uint(acc) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)cd.c));
@@ -143,10 +146,13 @@ __global__ void eval_rescore_kernel(const float *Q, const float *M, const tc::Ca
 // operation order per (question, word) as the re-score pass — tests hold the tensor-core pipeline to an identical
 // report against it.  scores = Q (nq x D) . M^T (D x words), 64 x 64 tile per CTA, 4 x 4 per thread, fused arg-max:
 // best[q] = max over c not in {b1,b2,b3} with score > 0 of (score, smallest c).
+// STORE = true (the top-k lists' fall-back, w2b_eval_topk.cuh): every score is stored instead, S[q * ldS + c] for
+// q < nq, c < words (Q and M then point at one block of queries and one chunk of the vocabulary); q3 and best unused.
 constexpr int TM = 64, TN = 64, TK = 16;
+template <bool STORE>
 __global__ void __launch_bounds__(256) eval_score_kernel(const float *Q, const float *M, const int *q3,
                                                          unsigned long long *best, long long nq, long long words,
-                                                         long long D, long long Dp) {
+                                                         long long D, long long Dp, float *S, long long ldS) {
   __shared__ float As[TK][TM + 4];
   __shared__ float Bs[TK][TN + 4];
   const int tid = threadIdx.x;
@@ -182,29 +188,41 @@ __global__ void __launch_bounds__(256) eval_score_kernel(const float *Q, const f
     }
     __syncthreads();
   }
+  if constexpr (STORE) {
 #pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const long long q = q0 + ty * 4 + i;
-    const bool qok = q < nq;  // no early exit: the shuffles below need the whole warp
-    const int b1 = qok ? q3[q * 3] : -1, b2 = qok ? q3[q * 3 + 1] : -1, b3 = qok ? q3[q * 3 + 2] : -1;
-    unsigned long long key = 0;
+    for (int i = 0; i < 4; ++i) {
+      const long long q = q0 + ty * 4 + i;
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const long long c = c0 + tx * 4 + j;
-      const float s = acc[i][j];
-      if (qok && c < words && c != b1 && c != b2 && c != b3 && s > 0.f) {
-        const unsigned long long k2 =
-            ((unsigned long long)__float_as_uint(s) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)c);
-        key = k2 > key ? k2 : key;
+      for (int j = 0; j < 4; ++j) {
+        const long long c = c0 + tx * 4 + j;
+        if (q < nq && c < words) S[q * ldS + c] = acc[i][j];
       }
     }
-    // combine the 16 threads of this row (same ty): lanes tx = 0..15 are contiguous in a half warp
+  } else {
 #pragma unroll
-    for (int o = 8; o > 0; o >>= 1) {
-      const unsigned long long other = __shfl_xor_sync(kFull, key, o);
-      key = other > key ? other : key;
+    for (int i = 0; i < 4; ++i) {
+      const long long q = q0 + ty * 4 + i;
+      const bool qok = q < nq;  // no early exit: the shuffles below need the whole warp
+      const int b1 = qok ? q3[q * 3] : -1, b2 = qok ? q3[q * 3 + 1] : -1, b3 = qok ? q3[q * 3 + 2] : -1;
+      unsigned long long key = 0;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const long long c = c0 + tx * 4 + j;
+        const float s = acc[i][j];
+        if (qok && c < words && c != b1 && c != b2 && c != b3 && s > 0.f) {
+          const unsigned long long k2 =
+              ((unsigned long long)__float_as_uint(s) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)c);
+          key = k2 > key ? k2 : key;
+        }
+      }
+      // combine the 16 threads of this row (same ty): lanes tx = 0..15 are contiguous in a half warp
+#pragma unroll
+      for (int o = 8; o > 0; o >>= 1) {
+        const unsigned long long other = __shfl_xor_sync(kFull, key, o);
+        key = other > key ? other : key;
+      }
+      if (tx == 0 && key && qok) atomicMax(best + q, key);
     }
-    if (tx == 0 && key && qok) atomicMax(best + q, key);
   }
 }
 
@@ -410,12 +428,12 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
         return W2B_ECUDA;
       }
       eval_qeps_kernel<<<(unsigned)((nq + 7) / 8), 256>>>(dQ, bqeps.as<float>(), nq, Dp);
-      CKE(cudaFuncSetAttribute(tc::eval_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
+      CKE(cudaFuncSetAttribute(tc::eval_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
       // x = question tile (fastest): the CTAs that share a 256-word tile of M run together, M streams from HBM once
       dim3 grid((unsigned)((nq + tc::BM - 1) / tc::BM), (unsigned)ntiles);
-      tc::eval_tc_kernel<<<grid, tc::THREADS, tc::SMEM_BYTES>>>(mapQ, mapM, dq3, bqeps.as<float>(), bgmax.as<unsigned>(),
+      tc::eval_tc_kernel<false><<<grid, tc::THREADS, tc::SMEM_BYTES>>>(mapQ, mapM, dq3, bqeps.as<float>(), bgmax.as<unsigned>(),
                                                                bcand.as<tc::Candidate>(), dcnt, cand_cap, (int)nq, (int)words,
-                                                               (int)Dp);
+                                                               (int)Dp, nullptr, 0);
       CKE(cudaGetLastError());
       CKE(cudaMemcpy(h_cnt, dcnt, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
       if (h_cnt[0] > cand_cap) {
@@ -429,7 +447,7 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
     if (need_simt) {
       CKE(cudaMemset(dbest, 0, nq * sizeof(unsigned long long)));
       dim3 grid((unsigned)((words + TN - 1) / TN), (unsigned)((nq + TM - 1) / TM));
-      eval_score_kernel<<<grid, 256>>>(dQ, dM, dq3, dbest, nq, words, size, Dp);
+      eval_score_kernel<false><<<grid, 256>>>(dQ, dM, dq3, dbest, nq, words, size, Dp, nullptr, 0);
     }
     CKE(cudaGetLastError());
     CKE(cudaEventRecord(e1.e));
@@ -538,11 +556,11 @@ extern "C" int w2b_eval_filter_scores(const float *Q, int64_t nq, const float *M
       return W2B_ECUDA;
     }
     eval_qeps_kernel<<<(unsigned)((nq + 7) / 8), 256>>>(bQ.as<float>(), bqeps.as<float>(), nq, Dp);
-    CKE(cudaFuncSetAttribute(tc::eval_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
+    CKE(cudaFuncSetAttribute(tc::eval_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
     dim3 grid((unsigned)((nq + tc::BM - 1) / tc::BM), (unsigned)((words + tc::BN - 1) / tc::BN));
-    tc::eval_tc_kernel<<<grid, tc::THREADS, tc::SMEM_BYTES>>>(mapQ, mapM, bq3.as<int>(), binf.as<float>(), bgmax.as<unsigned>(),
+    tc::eval_tc_kernel<false><<<grid, tc::THREADS, tc::SMEM_BYTES>>>(mapQ, mapM, bq3.as<int>(), binf.as<float>(), bgmax.as<unsigned>(),
                                                              bcand.as<tc::Candidate>(), bcnt.as<unsigned long long>(), cap,
-                                                             (int)nq, (int)words, (int)Dp);
+                                                             (int)nq, (int)words, (int)Dp, nullptr, 0);
     CKE(cudaGetLastError());
     unsigned long long n = 0;
     CKE(cudaMemcpy(&n, bcnt.p, sizeof n, cudaMemcpyDeviceToHost));
@@ -648,20 +666,26 @@ template <int BITS> int bits_filter(BitsState &st, int32_t *gram) {
 
 // Every score on the fp32 SIMT scorer: the planes become the fp32 table of the unpacked file, and
 // eval_normalize_kernel / eval_query_kernel / eval_score_kernel run as they do on a word2vec-binary file.
-template <int BITS> int bits_score_simt(BitsState &st, unsigned long long *dbest) {
-  const long long Dp = (st.D + tc::BK - 1) / tc::BK * tc::BK;
-  DevBuf bM, bQ;
+template <int BITS> int bits_fp32(BitsState &st, DevBuf &bM, DevBuf &bQ, long long Dp) {
   CKE(bM.alloc((size_t)st.V * Dp * sizeof(float)));
   CKE(bQ.alloc((size_t)st.nq * Dp * sizeof(float)));
   CKE(cudaMemset(bM.p, 0, (size_t)st.V * Dp * sizeof(float)));
   CKE(cudaMemset(bQ.p, 0, (size_t)st.nq * Dp * sizeof(float)));
-  CKE(cudaMemset(dbest, 0, st.nq * sizeof(unsigned long long)));
   bits::eval_bits_decode_kernel<BITS><<<(unsigned)((st.V * st.D + 255) / 256), 256>>>(
       st.sign.as<unsigned>(), st.mag.as<unsigned>(), bM.as<float>(), st.V, st.D, st.Wp, Dp);
   eval_normalize_kernel<<<(unsigned)((st.V + 7) / 8), 256>>>(bM.as<float>(), st.V, st.D, Dp, BITS);
   eval_query_kernel<<<(unsigned)((st.nq * st.D + 255) / 256), 256>>>(bM.as<float>(), st.q3.as<int>(), bQ.as<float>(), st.nq, st.D, Dp);
+  return W2B_OK;
+}
+
+template <int BITS> int bits_score_simt(BitsState &st, unsigned long long *dbest) {
+  const long long Dp = (st.D + tc::BK - 1) / tc::BK * tc::BK;
+  DevBuf bM, bQ;
+  CKE(cudaMemset(dbest, 0, st.nq * sizeof(unsigned long long)));
+  int rc = bits_fp32<BITS>(st, bM, bQ, Dp);
+  if (rc) return rc;
   dim3 grid((unsigned)((st.V + TN - 1) / TN), (unsigned)((st.nq + TM - 1) / TM));
-  eval_score_kernel<<<grid, 256>>>(bQ.as<float>(), bM.as<float>(), st.q3.as<int>(), dbest, st.nq, st.V, st.D, Dp);
+  eval_score_kernel<false><<<grid, 256>>>(bQ.as<float>(), bM.as<float>(), st.q3.as<int>(), dbest, st.nq, st.V, st.D, Dp, nullptr, 0);
   CKE(cudaGetLastError());
   CKE(cudaDeviceSynchronize());  // bM and bQ are freed on return
   return W2B_OK;
@@ -687,22 +711,23 @@ template <int BITS> int bits_answers(BitsState &st, bool simt, unsigned long lon
   return simt ? bits_score_simt<BITS>(st, dbest) : W2B_OK;
 }
 
-int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, const char *questions_file, int device,
-                                 w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers,
-                                 int64_t answers_cap, int64_t *n_questions) {
+// The rows and names of a packed file (the first `threshold` words when threshold > 0).
+int read_packed(const char *packed_file, int64_t threshold, std::vector<std::string> &names, std::vector<uint8_t> &rows,
+                long long &words, long long &size, int &bits) {
   w2b_packed_file pf;
   int rc = w2b_packed_open(packed_file, &pf);
   if (rc) return rc;
-  long long words = pf.V;
-  const long long size = pf.D;
+  words = pf.V;
+  size = pf.D;
+  bits = pf.bits;
   if (threshold > 0 && words > threshold) words = threshold;
   // D <= 2^17: the integer scores stay below 2^24 and eval_bits_qeps_kernel's slack holds
   if (words < 1 || words > 0x7fffffffLL || size > (1LL << 17) || words > (1LL << 40) / pf.nbytes) {
     w2b_set_error("bad header: %lld words of size %lld", words, size);
     return W2B_EIO;
   }
-  std::vector<std::string> names(words);
-  std::vector<uint8_t> rows((size_t)words * pf.nbytes);
+  names.resize(words);
+  rows.resize((size_t)words * pf.nbytes);
   for (long long b = 0; b < words; ++b) {
     char raw[256];
     rc = w2b_packed_next(&pf, raw, sizeof raw, &rows[(size_t)b * pf.nbytes]);
@@ -712,20 +737,35 @@ int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, con
       if (*p != '\n' && w.size() < 50) w.push_back(*p);
     names[b] = upper(w);
   }
+  return W2B_OK;
+}
+
+// the distinct query words: the Gram kernel runs once per word, not once per question
+void distinct_words(const std::vector<int> &q3, std::vector<int> &qid, std::vector<int> &q3w) {
+  q3w.resize(q3.size());
+  std::unordered_map<int, int> row_of;
+  for (size_t i = 0; i < q3.size(); ++i) {
+    auto it = row_of.emplace(q3[i], (int)qid.size());
+    if (it.second) qid.push_back(q3[i]);
+    q3w[i] = it.first->second;
+  }
+}
+
+int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, const char *questions_file, int device,
+                                 w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers,
+                                 int64_t answers_cap, int64_t *n_questions) {
+  std::vector<std::string> names;
+  std::vector<uint8_t> rows;
+  long long words = 0, size = 0;
+  int file_bits = 0;
+  int rc = read_packed(packed_file, threshold, names, rows, words, size, file_bits);
+  if (rc) return rc;
   Questions qs;
   rc = parse_questions(questions_file, names, qs);
   if (rc) return rc;
   const long long nq = (long long)qs.q3.size() / 3;
-  // the distinct query words: the Gram kernel runs once per word, not once per question
-  std::vector<int> qid, q3w(qs.q3.size());
-  {
-    std::unordered_map<int, int> row_of;
-    for (size_t i = 0; i < qs.q3.size(); ++i) {
-      auto it = row_of.emplace(qs.q3[i], (int)qid.size());
-      if (it.second) qid.push_back(qs.q3[i]);
-      q3w[i] = it.first->second;
-    }
-  }
+  std::vector<int> qid, q3w;
+  distinct_words(qs.q3, qid, q3w);
 
   std::vector<unsigned long long> best(nq > 0 ? nq : 1, 0);
   float ms = 0.f;
@@ -741,7 +781,7 @@ int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, con
     const bool simt = dbg && atoi(dbg) != 0;
     BitsState st;
     DevBuf bbest;
-    rc = bits_upload(st, rows.data(), words, (int)size, pf.bits, qid.data(), (int)qid.size(), q3w.data(), qs.q3.data(), nq,
+    rc = bits_upload(st, rows.data(), words, (int)size, file_bits, qid.data(), (int)qid.size(), q3w.data(), qs.q3.data(), nq,
                      (unsigned long long)nq * 1024ull);  // the cap of the tensor-core filter's list
     if (rc) return rc;
     CKE(bbest.alloc(nq * sizeof(unsigned long long)));
@@ -751,7 +791,7 @@ int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, con
     CKE(cudaEventCreate(&e1.e));
     CKE(cudaEventRecord(e0.e));
     unsigned long long counts[2] = {0, 0};
-    rc = pf.bits == 1 ? bits_answers<1>(st, simt, bbest.as<unsigned long long>(), counts)
+    rc = file_bits == 1 ? bits_answers<1>(st, simt, bbest.as<unsigned long long>(), counts)
                       : bits_answers<2>(st, simt, bbest.as<unsigned long long>(), counts);
     if (rc) return rc;
     CKE(cudaEventRecord(e1.e));
@@ -838,5 +878,392 @@ extern "C" int w2b_eval_packed_scores(const uint8_t *rows, int64_t V, int64_t D,
       for (const tc::Candidate &c : cand) approx[(size_t)c.q * V + c.c] = c.s;
     }
     return W2B_OK;
+  });
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Top-k lists (w2b_analogy_topk, w2b_nearest; kernels in w2b_eval_topk.cuh).  A query is an analogy question or a
+// nearest-neighbour word w taken as the question (w, w, w): vec = (M[w] - M[w]) + M[w] = M[w] exactly, and only w is
+// skipped.  The vocabulary is walked a chunk at a time; a chunk of scores for a block of queries is written densely
+// (kDenseFloats floats at most) and read by the selection kernel, which carries every query's kept set to the next
+// chunk.  Approximate scores (TF32, or the bit domain of a packed file) leave a candidate list per query that is
+// re-scored exactly; a list that overflows, and W2B_EVAL_SIMT=1, take exact fp32 scores from the SIMT scorer instead
+// and select with 64-bit keys.
+namespace {
+
+constexpr long long kDenseFloats = 8ll << 20;  // a chunk of scores: 32 MB
+constexpr long long kListBytes = 2ll << 30;     // candidate lists, keys, kept sets and lists of one batch of queries
+
+struct TopkBufs {
+  DevBuf kept, kth, cand, ncand, keys, ids, scores, cnt, S;
+  long long nq = 0, nqb = 0, ch = 0, chunks = 0;
+  int k = 0, cap = 0;
+};
+
+// queries per block and words per chunk of the dense score buffer
+void dense_geometry(TopkBufs &b, long long words, long long max_ch) {
+  b.nqb = std::min<long long>(b.nq, 1024);
+  b.ch = std::max<long long>(256, kDenseFloats / b.nqb / 256 * 256);
+  b.ch = std::min(b.ch, std::min(max_ch, (words + 255) / 256 * 256));
+}
+
+int topk_alloc(TopkBufs &b, long long nq, int k) {
+  b.nq = nq;
+  b.k = k;
+  // candidates a query may have: its k and what ties within 2 eps of them, plus what each chunk adds above a
+  // threshold that is still rising (about k ln(chunks) over a walk of the vocabulary, measured at 20 chunks)
+  b.cap = 8 * k + 1024;
+  CKE(b.kept.alloc((size_t)nq * k * 8));
+  CKE(b.kth.alloc((size_t)nq * 8));
+  CKE(b.cand.alloc((size_t)nq * b.cap * sizeof(topk::Cand)));
+  CKE(b.ncand.alloc((size_t)nq * 4));
+  CKE(b.keys.alloc((size_t)nq * b.cap * 8));
+  CKE(b.ids.alloc((size_t)nq * k * 4));
+  CKE(b.scores.alloc((size_t)nq * k * 4));
+  CKE(b.cnt.alloc(8));
+  CKE(cudaMemset(b.ncand.p, 0, (size_t)nq * 4));
+  CKE(cudaMemset(b.cnt.p, 0, 8));
+  return W2B_OK;
+}
+
+int topk_reset(TopkBufs &b) {  // empty kept sets
+  CKE(cudaMemset(b.kept.p, 0, (size_t)b.nq * b.k * 8));
+  CKE(cudaMemset(b.kth.p, 0, (size_t)b.nq * 8));
+  b.chunks = 0;
+  return W2B_OK;
+}
+
+template <bool EXACT> int topk_select(TopkBufs &b, long long qb, long long nqb, long long c0, int nc, const int *dq3,
+                                      const float *dqeps) {
+  using K = typename std::conditional<EXACT, unsigned long long, unsigned>::type;
+  topk::topk_select_kernel<EXACT><<<(unsigned)nqb, topk::THREADS>>>(
+      b.S.as<float>(), b.ch, c0, nc, dq3 + 3 * qb, EXACT ? nullptr : dqeps + qb, b.kept.as<K>() + qb * b.k,
+      b.kth.as<K>() + qb, EXACT ? nullptr : b.cand.as<topk::Cand>() + qb * b.cap, EXACT ? nullptr : b.ncand.as<int>() + qb,
+      b.cap, b.k);
+  CKE(cudaGetLastError());
+  return W2B_OK;
+}
+
+// exact lists from the SIMT scorer: Q (nq x Dp) against M (words x Dp), both normalised fp32
+int topk_simt(TopkBufs &b, const float *dQ, const float *dM, const int *dq3, long long words, long long D, long long Dp) {
+  int rc = topk_reset(b);
+  if (rc) return rc;
+  for (long long c0 = 0; c0 < words; c0 += b.ch, ++b.chunks) {
+    const int nc = (int)std::min(b.ch, words - c0);
+    for (long long qb = 0; qb < b.nq; qb += b.nqb) {
+      const long long n = std::min(b.nqb, b.nq - qb);
+      dim3 grid((unsigned)((nc + TN - 1) / TN), (unsigned)((n + TM - 1) / TM));
+      eval_score_kernel<true><<<grid, 256>>>(dQ + qb * Dp, dM + c0 * Dp, nullptr, nullptr, n, nc, D, Dp, b.S.as<float>(), b.ch);
+      if ((rc = topk_select<true>(b, qb, n, c0, nc, dq3, nullptr))) return rc;
+    }
+  }
+  topk::topk_final_kernel<<<(unsigned)b.nq, topk::THREADS>>>(b.kept.as<unsigned long long>(), nullptr, b.k, b.k,
+                                                             b.ids.as<int>(), b.scores.as<float>());
+  CKE(cudaGetLastError());
+  return W2B_OK;
+}
+
+// after a filter pass: true when some query's candidate list overflowed
+int topk_overflowed(TopkBufs &b, bool &over, int64_t &candidates) {
+  std::vector<int> n((size_t)b.nq);
+  CKE(cudaMemcpy(n.data(), b.ncand.p, (size_t)b.nq * 4, cudaMemcpyDeviceToHost));
+  over = false;
+  for (int x : n) {
+    over |= x > b.cap;
+    candidates += x;
+  }
+  return W2B_OK;
+}
+
+int topk_final(TopkBufs &b) {
+  topk::topk_final_kernel<<<(unsigned)b.nq, topk::THREADS>>>(b.keys.as<unsigned long long>(), b.ncand.as<int>(), b.cap,
+                                                             b.k, b.ids.as<int>(), b.scores.as<float>());
+  CKE(cudaGetLastError());
+  return W2B_OK;
+}
+
+// fp32 file: the queries of one batch against the normalised table dM, TF32 filter + exact re-score (or the SIMT
+// scorer).  *ms += the device time from the first kernel to the last (uploads and frees outside it).
+int topk_fp32(const float *dM, long long words, long long size, const std::vector<int> &q3, bool simt, TopkBufs &b,
+              w2b_topk_stats &s, float *ms) {
+  const long long nq = b.nq, Dp = (size + tc::BK - 1) / tc::BK * tc::BK;
+  DevBuf bQ, bq3, bqeps;
+  DevEvent e0, e1;
+  CKE(bQ.alloc((size_t)nq * Dp * sizeof(float)));
+  CKE(bq3.alloc(q3.size() * sizeof(int)));
+  CKE(bqeps.alloc(nq * sizeof(float)));
+  float *dQ = bQ.as<float>();
+  int *dq3 = bq3.as<int>();
+  CKE(cudaMemset(dQ, 0, (size_t)nq * Dp * sizeof(float)));
+  CKE(cudaMemcpy(dq3, q3.data(), q3.size() * sizeof(int), cudaMemcpyHostToDevice));
+  dense_geometry(b, words, 1LL << 40);
+  CKE(b.S.alloc((size_t)b.nqb * b.ch * sizeof(float)));
+  CKE(cudaEventCreate(&e0.e));
+  CKE(cudaEventCreate(&e1.e));
+  CKE(cudaEventRecord(e0.e));
+  eval_query_kernel<<<(unsigned)((nq * size + 255) / 256), 256>>>(dM, dq3, dQ, nq, size, Dp);
+  int rc = W2B_OK;
+  if (!simt) {
+    if ((rc = topk_reset(b))) return rc;
+    if (rc) return rc;
+    eval_qeps_kernel<<<(unsigned)((nq + 7) / 8), 256>>>(dQ, bqeps.as<float>(), nq, Dp);
+    CKE(cudaFuncSetAttribute(tc::eval_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc::SMEM_BYTES));
+    std::vector<CUtensorMap> mapQ((size_t)((nq + b.nqb - 1) / b.nqb));  // one per block of queries
+    for (size_t i = 0; i < mapQ.size(); ++i)
+      if (!tc::make_map(&mapQ[i], dQ + (long long)i * b.nqb * Dp, std::min(b.nqb, nq - (long long)i * b.nqb), Dp, tc::BM)) {
+        w2b_set_error("cuTensorMapEncodeTiled failed (driver too old for TMA?)");
+        return W2B_ECUDA;
+      }
+    for (long long c0 = 0; c0 < words; c0 += b.ch, ++b.chunks) {
+      const int nc = (int)std::min(b.ch, words - c0);
+      CUtensorMap mapM;
+      if (!tc::make_map(&mapM, dM + c0 * Dp, nc, Dp, tc::BN)) {
+        w2b_set_error("cuTensorMapEncodeTiled failed (driver too old for TMA?)");
+        return W2B_ECUDA;
+      }
+      for (long long qb = 0; qb < nq; qb += b.nqb) {
+        const long long n = std::min(b.nqb, nq - qb);
+        dim3 grid((unsigned)((n + tc::BM - 1) / tc::BM), (unsigned)((nc + tc::BN - 1) / tc::BN));
+        tc::eval_tc_kernel<true><<<grid, tc::THREADS, tc::SMEM_BYTES>>>(mapQ[qb / b.nqb], mapM, nullptr, nullptr, nullptr, nullptr,
+                                                                       nullptr, 0, (int)n, nc, (int)Dp, b.S.as<float>(), b.ch);
+        if ((rc = topk_select<false>(b, qb, n, c0, nc, dq3, bqeps.as<float>()))) return rc;
+      }
+    }
+    bool over = false;
+    if ((rc = topk_overflowed(b, over, s.candidates))) return rc;
+    if (over) {
+      simt = true;  // ties by the thousand (e.g. all vectors equal): every score exactly instead
+    } else {
+      topk::topk_rescore_kernel<<<(unsigned)((nq * b.cap + 127) / 128), 128>>>(
+          dQ, dM, b.cand.as<topk::Cand>(), b.ncand.as<int>(), b.cap, b.kth.as<unsigned>(), bqeps.as<float>(),
+          b.keys.as<unsigned long long>(), b.cnt.as<unsigned long long>(), nq, (int)size, Dp);
+      if ((rc = topk_final(b))) return rc;
+    }
+  }
+  s.simt |= simt;
+  if (simt && (rc = topk_simt(b, dQ, dM, dq3, words, size, Dp))) return rc;
+  CKE(cudaEventRecord(e1.e));
+  CKE(cudaEventSynchronize(e1.e));  // bQ, bq3 and bqeps are freed on return
+  float t = 0.f;
+  CKE(cudaEventElapsedTime(&t, e0.e, e1.e));
+  *ms += t;
+  return W2B_OK;
+}
+
+// packed file: planes, then per chunk the Gram kernel and the bit-domain scores of every block of queries
+template <int BITS> int topk_packed_run(BitsState &st, bool simt, TopkBufs &b, w2b_topk_stats &s) {
+  int rc = bits_planes<BITS>(st);
+  if (rc) return rc;
+  const long long nq = b.nq;
+  if (!simt) {
+    if ((rc = topk_reset(b))) return rc;
+    b.nqb = std::max<long long>(1, std::min(nq, kDenseFloats / st.chunk));
+    b.ch = st.chunk;
+    CKE(b.S.alloc((size_t)b.nqb * b.ch * sizeof(float)));
+    for (long long c0 = 0; c0 < st.V; c0 += st.chunk, ++b.chunks) {
+      const int nc = (int)std::min(st.chunk, st.V - c0);
+      dim3 gg((unsigned)((nc + bits::GT - 1) / bits::GT), (unsigned)((st.W + bits::GT - 1) / bits::GT));
+      bits::eval_bits_gram_kernel<BITS><<<gg, 256>>>(st.sign.as<unsigned>(), st.mag.as<unsigned>(), st.hpop.as<int>(),
+                                                    st.qid.as<int>(), st.W, c0, nc, st.D, st.Wp, st.G.as<int>(), st.chunk);
+      for (long long qb = 0; qb < nq; qb += b.nqb) {
+        const long long n = std::min(b.nqb, nq - qb);
+        bits::eval_bits_combine_store_kernel<<<dim3((unsigned)((nc + 255) / 256), (unsigned)n), 256>>>(
+            st.G.as<int>(), st.chunk, c0, nc, st.ilen.as<float>(), st.q3w.as<int>() + 3 * qb, st.qk.as<float>() + 3 * qb,
+            b.S.as<float>(), b.ch);
+        if ((rc = topk_select<false>(b, qb, n, c0, nc, st.q3.as<int>(), st.qeps.as<float>()))) return rc;
+      }
+    }
+    bool over = false;
+    if ((rc = topk_overflowed(b, over, s.candidates))) return rc;
+    if (over) {
+      simt = true;
+    } else {
+      topk::topk_bits_rescore_kernel<BITS><<<(unsigned)((nq * b.cap + 127) / 128), 128>>>(
+          st.sign.as<unsigned>(), st.mag.as<unsigned>(), st.len.as<float>(), st.q3.as<int>(), b.cand.as<topk::Cand>(),
+          b.ncand.as<int>(), b.cap, b.kth.as<unsigned>(), st.qeps.as<float>(), b.keys.as<unsigned long long>(),
+          b.cnt.as<unsigned long long>(), nq, st.D, st.Wp);
+      return topk_final(b);
+    }
+  }
+  s.simt = 1;
+  const long long Dp = (st.D + tc::BK - 1) / tc::BK * tc::BK;
+  DevBuf bM, bQ;
+  if ((rc = bits_fp32<BITS>(st, bM, bQ, Dp))) return rc;
+  dense_geometry(b, st.V, 1LL << 40);
+  b.S.reset();  // the filter's chunk had another shape
+  CKE(b.S.alloc((size_t)b.nqb * b.ch * sizeof(float)));
+  if ((rc = topk_simt(b, bQ.as<float>(), bM.as<float>(), st.q3.as<int>(), st.V, st.D, Dp))) return rc;
+  CKE(cudaDeviceSynchronize());  // bM and bQ are freed on return
+  return W2B_OK;
+}
+
+// the packed pipeline of one batch, timed from the plane kernel on (as the arg-max evaluator times it)
+template <int BITS> int topk_packed(BitsState &st, bool simt, TopkBufs &b, w2b_topk_stats &s, float *ms) {
+  DevEvent e0, e1;
+  CKE(cudaEventCreate(&e0.e));
+  CKE(cudaEventCreate(&e1.e));
+  CKE(cudaEventRecord(e0.e));
+  int rc = topk_packed_run<BITS>(st, simt, b, s);
+  if (rc) return rc;
+  CKE(cudaEventRecord(e1.e));
+  CKE(cudaEventSynchronize(e1.e));
+  float t = 0.f;
+  CKE(cudaEventElapsedTime(&t, e0.e, e1.e));
+  *ms += t;
+  return W2B_OK;
+}
+
+// bit level of a packed file (three integers on its first line, as accuracy_main.cpp tells them apart), else 0
+int packed_bits_of(const char *path) {
+  long long words, size, bits = 0;
+  char line[128], extra;
+  if (FILE *f = fopen(path, "rb")) {
+    if (!fgets(line, sizeof line, f) || sscanf(line, "%lld %lld %lld %c", &words, &size, &bits, &extra) != 3) bits = 0;
+    fclose(f);
+  }
+  return (int)bits;
+}
+
+int topk_impl(const char *vectors_file, int bitlevel, int64_t threshold, bool nearest, const char *input, int k,
+              int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries, w2b_topk_stats *stats) {
+  w2b_topk_stats s;
+  memset(&s, 0, sizeof s);
+  const int packed = packed_bits_of(vectors_file);
+  if (packed && bitlevel != 0 && bitlevel != packed) {
+    w2b_set_error("%s holds %d-bit vectors: bitlevel must be %d or 0", vectors_file, packed, packed);
+    return W2B_EINVAL;
+  }
+  std::vector<std::string> names;
+  std::vector<float> M;
+  std::vector<uint8_t> rows;
+  long long words = 0, size = 0;
+  int file_bits = 0;
+  int rc = W2B_OK;
+  if (cap_queries > 0) {  // (counting the queries needs no vectors: no word is then in the vocabulary)
+    rc = packed ? read_packed(vectors_file, threshold, names, rows, words, size, file_bits)
+                : read_vectors(vectors_file, threshold, names, M, words, size);
+    if (rc) return rc;
+  }
+  // per output row (file order): the query it is, or -1 (a word is not in the vocabulary)
+  std::vector<int> q3, row_q;
+  if (nearest) {
+    std::unordered_map<std::string, int> first;  // first match, as parse_questions finds words
+    for (long long w = words - 1; w >= 0; --w) first[names[w]] = (int)w;
+    FILE *f = input ? fopen(input, "rb") : stdin;
+    if (!f) { w2b_set_error("words file not found"); return W2B_EIO; }
+    FileCloser closer{f};
+    char buf[2048];
+    while (fscanf(f, "%2000s", buf) == 1) {
+      auto it = first.find(upper(buf));
+      row_q.push_back(it == first.end() ? -1 : (int)(q3.size() / 3));
+      if (it != first.end()) q3.insert(q3.end(), {it->second, it->second, it->second});
+    }
+  } else {
+    Questions qs;
+    if ((rc = parse_questions(input, names, qs))) return rc;
+    for (const Ev &e : qs.events)
+      if (e.kind == 1) row_q.push_back(e.qidx);
+    q3 = qs.q3;
+  }
+  const long long nq = (long long)q3.size() / 3;
+  s.queries = (int64_t)row_q.size();
+  s.skipped = s.queries - nq;
+  s.packed = packed != 0;
+  std::vector<int32_t> hid((size_t)nq * k);
+  std::vector<float> hsc((size_t)nq * k);
+  if (nq > 0 && cap_queries > 0) {
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || device >= ndev) {
+      w2b_set_error("no CUDA device %d: the evaluator has no CPU fallback", device);
+      return W2B_ECUDA;
+    }
+    CKE(cudaSetDevice(device));
+    const char *dbg = getenv("W2B_EVAL_SIMT");
+    const bool simt = dbg && atoi(dbg) != 0;
+    // fp32 table: uploaded and normalised once for every batch
+    DevBuf bM;
+    const long long Dp = (size + tc::BK - 1) / tc::BK * tc::BK;
+    if (!packed) {
+      DevEvent e0, e1;
+      CKE(bM.alloc((size_t)words * Dp * sizeof(float)));
+      CKE(cudaMemset(bM.p, 0, (size_t)words * Dp * sizeof(float)));
+      CKE(cudaMemcpy2D(bM.p, Dp * sizeof(float), M.data(), size * sizeof(float), size * sizeof(float), words,
+                       cudaMemcpyHostToDevice));
+      CKE(cudaEventCreate(&e0.e));
+      CKE(cudaEventCreate(&e1.e));
+      CKE(cudaEventRecord(e0.e));
+      eval_normalize_kernel<<<(unsigned)((words + 7) / 8), 256>>>(bM.as<float>(), words, size, Dp, bitlevel);
+      CKE(cudaEventRecord(e1.e));
+      CKE(cudaEventSynchronize(e1.e));
+      CKE(cudaEventElapsedTime(&s.gpu_ms, e0.e, e1.e));
+    }
+    // queries in batches, so that candidate lists and kept sets stay within kListBytes
+    const long long per_query = (8LL * k + 1024) * 16 + 16LL * k + 16;
+    const long long batch = std::max<long long>(1024, kListBytes / per_query);
+    for (long long q0 = 0; q0 < nq; q0 += batch) {
+      const long long nb = std::min(batch, nq - q0);
+      const std::vector<int> sub(q3.begin() + 3 * q0, q3.begin() + 3 * (q0 + nb));
+      TopkBufs b;
+      if ((rc = topk_alloc(b, nb, k))) return rc;
+      if (!packed) {
+        rc = topk_fp32(bM.as<float>(), words, size, sub, simt, b, s, &s.gpu_ms);
+      } else {
+        BitsState st;
+        std::vector<int> qid, q3w;
+        distinct_words(sub, qid, q3w);
+        if ((rc = bits_upload(st, rows.data(), words, (int)size, file_bits, qid.data(), (int)qid.size(), q3w.data(),
+                              sub.data(), nb, 1)))  // (its arg-max candidate list is not used)
+          return rc;
+        rc = file_bits == 1 ? topk_packed<1>(st, simt, b, s, &s.gpu_ms) : topk_packed<2>(st, simt, b, s, &s.gpu_ms);
+      }
+      if (rc) return rc;
+      CKE(cudaMemcpy(hid.data() + q0 * k, b.ids.p, (size_t)nb * k * 4, cudaMemcpyDeviceToHost));
+      CKE(cudaMemcpy(hsc.data() + q0 * k, b.scores.p, (size_t)nb * k * 4, cudaMemcpyDeviceToHost));
+      unsigned long long n_rescored = 0;
+      CKE(cudaMemcpy(&n_rescored, b.cnt.p, 8, cudaMemcpyDeviceToHost));
+      s.rescored += (int64_t)n_rescored;
+      s.chunks = std::max<int64_t>(s.chunks, b.chunks);
+    }
+  }
+  for (size_t r = 0; r < row_q.size() && (int64_t)r < cap_queries; ++r)
+    for (int j = 0; j < k; ++j) {
+      const int q = row_q[r];
+      ids[r * k + j] = q >= 0 ? hid[(size_t)q * k + j] : -1;
+      scores[r * k + j] = q >= 0 ? hsc[(size_t)q * k + j] : 0.f;
+    }
+  if (n_queries) *n_queries = (int64_t)row_q.size();
+  if (stats) *stats = s;
+  return W2B_OK;
+}
+
+int topk_args(const char *who, const char *vectors_file, int k, const int32_t *ids, const float *scores,
+              int64_t cap_queries) {
+  if (!vectors_file || k < 1 || k > W2B_MAX_TOPK || cap_queries < 0 || (cap_queries > 0 && (!ids || !scores))) {
+    w2b_set_error("%s: bad arguments (vectors_file %s, k = %d: 1 <= k <= %d, ids and scores for %lld rows)", who,
+                  vectors_file ? "set" : "NULL", k, W2B_MAX_TOPK, (long long)cap_queries);
+    return W2B_EINVAL;
+  }
+  return W2B_OK;
+}
+
+}  // namespace
+
+extern "C" int w2b_analogy_topk(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file,
+                                int k, int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries,
+                                w2b_topk_stats *st) {
+  if (int rc = topk_args("w2b_analogy_topk", vectors_file, k, ids, scores, cap_queries)) return rc;
+  return no_throw("w2b_analogy_topk", [&] {
+    return topk_impl(vectors_file, bitlevel, threshold, false, questions_file, k, device, ids, scores, cap_queries,
+                     n_queries, st);
+  });
+}
+
+extern "C" int w2b_nearest(const char *vectors_file, int bitlevel, int64_t threshold, const char *words_file, int k,
+                           int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries,
+                           w2b_topk_stats *st) {
+  if (int rc = topk_args("w2b_nearest", vectors_file, k, ids, scores, cap_queries)) return rc;
+  return no_throw("w2b_nearest", [&] {
+    return topk_impl(vectors_file, bitlevel, threshold, true, words_file, k, device, ids, scores, cap_queries, n_queries,
+                     st);
   });
 }

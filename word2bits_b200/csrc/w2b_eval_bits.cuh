@@ -221,6 +221,10 @@ __global__ void eval_bits_qeps_kernel(const unsigned *sign, const unsigned *mag,
 // above 0 can have an approximate score <= 0) and s >= running best - 2 eps.  q3 = the question's three vocabulary
 // ids (skipped as answers; -1 = none), q3w = their rows of G.
 constexpr int CT = 1024, CPL = CT / 32;
+__device__ __forceinline__ float combine(int g1, int g2, int g3, float k1, float k2, float k3, float ilen) {
+  const float t1 = __fmul_rn((float)g1, k1);
+  return __fmul_rn(__fmaf_rn((float)g3, k3, __fmaf_rn((float)g2, k2, -t1)), ilen);
+}
 __global__ void __launch_bounds__(256) eval_bits_combine_kernel(const int *G, long long ldg, long long c0, int nc,
                                                                 const float *ilen, const int *q3, const int *q3w,
                                                                 const float *qk, const float *qeps, unsigned *gmax,
@@ -242,8 +246,7 @@ __global__ void __launch_bounds__(256) eval_bits_combine_kernel(const int *G, lo
     const long long c = c0 + t;
     s[i] = -INFINITY;  // not a competitor
     if (t < nc && c != b1 && c != b2 && c != b3) {
-      const float t1 = __fmul_rn((float)g1[t], k1);
-      s[i] = __fmul_rn(__fmaf_rn((float)g3[t], k3, __fmaf_rn((float)g2[t], k2, -t1)), ilen[c]);
+      s[i] = combine(g1[t], g2[t], g3[t], k1, k2, k3, ilen[c]);
       best = fmaxf(best, s[i]);
     }
   }
@@ -260,22 +263,22 @@ __global__ void __launch_bounds__(256) eval_bits_combine_kernel(const int *G, lo
     }
 }
 
-// Exact scores of the surviving candidates, the packed counterpart of eval_rescore_kernel: a candidate still within
-// 2 eps of the question's final best is scored as src/compute-accuracy.c:155-165 does on the unpacked file,
-// m = level / len (a row has one or two magnitudes: the quotients are taken once per row, the sign is exact),
-// vec[a] = (m2[a] - m1[a]) + m3[a], dist += vec[a] * m_c[a] with the product rounded, then added, a ascending; and
-// competes under the reference's rule: strictly positive, larger score wins, smaller index on ties.
+// The same scores stored densely, for the top-k selection (w2b_eval_topk.cuh): S[q * ldS + t] = the filter's score
+// of question q against word c0 + t, t < nc, every word (the selection skips the query words).
+__global__ void __launch_bounds__(256) eval_bits_combine_store_kernel(const int *G, long long ldg, long long c0, int nc,
+                                                                      const float *ilen, const int *q3w, const float *qk,
+                                                                      float *S, long long ldS) {
+  const int q = blockIdx.y, t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nc) return;
+  const int w1 = q3w[q * 3], w2 = q3w[q * 3 + 1], w3 = q3w[q * 3 + 2];
+  S[(long long)q * ldS + t] = combine(G[w1 * ldg + t], G[w2 * ldg + t], G[w3 * ldg + t], qk[q * 3], qk[q * 3 + 1],
+                                      qk[q * 3 + 2], ilen[c0 + t]);
+}
+
+// dist of one packed candidate: r = its question's three rows and the candidate's row (see eval_bits_rescore_kernel)
 template <int BITS>
-__global__ void eval_bits_rescore_kernel(const unsigned *sign, const unsigned *mag, const float *len, const int *q3,
-                                         const tc::Candidate *cand, unsigned long long n_cand, const float *qeps,
-                                         const unsigned *gmax, unsigned long long *best, unsigned long long *n_rescored,
-                                         int D, int Wp) {
-  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_cand) return;
-  const tc::Candidate cd = cand[i];
-  const unsigned g = gmax[cd.q];
-  if (!(cd.s >= __uint_as_float(g & 0x7fffffffu) - 2.f * qeps[cd.q])) return;
-  const long long r[4] = {q3[cd.q * 3], q3[cd.q * 3 + 1], q3[cd.q * 3 + 2], cd.c};
+__device__ __forceinline__ float exact_score(const unsigned *sign, const unsigned *mag, const float *len,
+                                             const long long (&r)[4], int D, int Wp) {
   float lo[4], hi[4];  // the row's quotients for the small (or only) and the large magnitude
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
@@ -302,6 +305,26 @@ __global__ void eval_bits_rescore_kernel(const unsigned *sign, const unsigned *m
       acc = __fadd_rn(acc, __fmul_rn(__fadd_rn(__fsub_rn(m[1], m[0]), m[2]), m[3]));
     }
   }
+  return acc;
+}
+
+// Exact scores of the surviving candidates, the packed counterpart of eval_rescore_kernel: a candidate still within
+// 2 eps of the question's final best is scored as src/compute-accuracy.c:155-165 does on the unpacked file,
+// m = level / len (a row has one or two magnitudes: the quotients are taken once per row, the sign is exact),
+// vec[a] = (m2[a] - m1[a]) + m3[a], dist += vec[a] * m_c[a] with the product rounded, then added, a ascending; and
+// competes under the reference's rule: strictly positive, larger score wins, smaller index on ties.
+template <int BITS>
+__global__ void eval_bits_rescore_kernel(const unsigned *sign, const unsigned *mag, const float *len, const int *q3,
+                                         const tc::Candidate *cand, unsigned long long n_cand, const float *qeps,
+                                         const unsigned *gmax, unsigned long long *best, unsigned long long *n_rescored,
+                                         int D, int Wp) {
+  const unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_cand) return;
+  const tc::Candidate cd = cand[i];
+  const unsigned g = gmax[cd.q];
+  if (!(cd.s >= __uint_as_float(g & 0x7fffffffu) - 2.f * qeps[cd.q])) return;
+  const long long r[4] = {q3[cd.q * 3], q3[cd.q * 3 + 1], q3[cd.q * 3 + 2], cd.c};
+  const float acc = exact_score<BITS>(sign, mag, len, r, D, Wp);
   atomicAdd(n_rescored, 1ull);
   if (acc > 0.f)
     atomicMax(best + cd.q, ((unsigned long long)__float_as_uint(acc) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)cd.c));

@@ -102,10 +102,14 @@ struct Candidate { int q, c; float s; };
 // positive).  cand[0 .. *n_cand) = every (q, c, approximate score) that was within 2*qeps[q] of the running best
 // its thread had seen when the score was read (a superset of what is within 2*qeps[q] of the final best); entries
 // beyond cand_cap are dropped and *n_cand keeps counting (the caller checks for overflow).
+// DENSE = true (the top-k lists, w2b_eval_topk.cuh): the epilogue only stores every TF32 score, S[q * ldS + c] for
+// q < nq, c < words (mapQ / mapM then cover one block of queries and one chunk of the vocabulary); q3, qeps, gmax and
+// the candidate list are not used.
+template <bool DENSE>
 __global__ void __launch_bounds__(THREADS, 1)
 eval_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapM, const int *q3,
                const float *qeps, unsigned *gmax, Candidate *cand, unsigned long long *n_cand, unsigned long long cand_cap,
-               int nq, int words, int Dp) {
+               int nq, int words, int Dp, float *S, long long ldS) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char *smem = (unsigned char *)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char *sA = smem, *sB = smem + STAGES * A_BYTES;
@@ -153,40 +157,56 @@ eval_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__
 
   // ---- epilogue.  Accumulator layout of m64nN: thread t holds rows 16*(t/32) + (t%32)/4 (+8) and, per 8-column
   // block j, columns 8j + 2*(t%4) (+1): d[4j + 2h + e] = (row + 8h, col + e).
+  if constexpr (DENSE) {
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int row = wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h, q = m0 + row;
-    const bool qok = q < nq;
-    const int b1 = qok ? q3[q * 3] : -1, b2 = qok ? q3[q * 3 + 1] : -1, b3 = qok ? q3[q * 3 + 2] : -1;
-    // lower bound for candidates: the question's best so far (any tile, any CTA) minus the error window
-    float thr = 0.f, eps2 = 0.f;
-    if (qok) {
-      const unsigned g = *(volatile unsigned *)(gmax + q);
-      eps2 = 2.f * qeps[q];
-      thr = (g ? __uint_as_float(g & 0x7fffffffu) : 0.f) - eps2;
+    for (int h = 0; h < 2; ++h) {
+      const int q = m0 + wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h;
+      if (q >= nq) continue;
+      float *srow = S + (long long)q * ldS;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = n0 + 8 * j + 2 * (t & 3) + e;
+          if (c < words) srow[c] = d[4 * j + 2 * h + e];
+        }
     }
-    float best = 0.f;
+  } else {
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
+    for (int h = 0; h < 2; ++h) {
+      const int row = wg * 64 + 16 * (t >> 5) + ((t & 31) >> 2) + 8 * h, q = m0 + row;
+      const bool qok = q < nq;
+      const int b1 = qok ? q3[q * 3] : -1, b2 = qok ? q3[q * 3 + 1] : -1, b3 = qok ? q3[q * 3 + 2] : -1;
+      // lower bound for candidates: the question's best so far (any tile, any CTA) minus the error window
+      float thr = 0.f, eps2 = 0.f;
+      if (qok) {
+        const unsigned g = *(volatile unsigned *)(gmax + q);
+        eps2 = 2.f * qeps[q];
+        thr = (g ? __uint_as_float(g & 0x7fffffffu) : 0.f) - eps2;
+      }
+      float best = 0.f;
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int c = n0 + 8 * j + 2 * (t & 3) + e;
-        const float s = d[4 * j + 2 * h + e];
-        // s > -eps2, not s > 0: a word whose exact score is a little above 0 can have an approximate score <= 0
-        if (qok && c < words && c != b1 && c != b2 && c != b3 && s > -eps2 && s >= thr) {
-          if (s > best) {
-            best = s;
-            thr = fmaxf(thr, s - eps2);  // (a superset is fine: thr only ever rises)
+      for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = n0 + 8 * j + 2 * (t & 3) + e;
+          const float s = d[4 * j + 2 * h + e];
+          // s > -eps2, not s > 0: a word whose exact score is a little above 0 can have an approximate score <= 0
+          if (qok && c < words && c != b1 && c != b2 && c != b3 && s > -eps2 && s >= thr) {
+            if (s > best) {
+              best = s;
+              thr = fmaxf(thr, s - eps2);  // (a superset is fine: thr only ever rises)
+            }
+            const unsigned long long at = atomicAdd(n_cand, 1ull);
+            if (at < cand_cap) cand[at] = Candidate{q, c, s};
           }
-          const unsigned long long at = atomicAdd(n_cand, 1ull);
-          if (at < cand_cap) cand[at] = Candidate{q, c, s};
         }
       }
+      // the four threads of a row hold disjoint columns: one atomic per row
+      best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, 1));
+      best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, 2));
+      if (qok && (t & 3) == 0 && best > 0.f) atomicMax(gmax + q, ordered(best));
     }
-    // the four threads of a row hold disjoint columns: one atomic per row
-    best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, 1));
-    best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, 2));
-    if (qok && (t & 3) == 0 && best > 0.f) atomicMax(gmax + q, ordered(best));
   }
 }
 
