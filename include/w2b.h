@@ -298,6 +298,27 @@ int w2b_nearest(const char *vectors_file, int bitlevel, int64_t threshold, const
                 int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries,
                 w2b_topk_stats *st);
 
+/* The evaluator on a context's own tables: the vectors are quantize(u+v) as w2b_export computes them (the file
+ * -binary 1 would write), with words[i] the name of row i (ctx's vocab_size names, the order of the rows).  Same
+ * arguments, report text, answers, lists and statistics as the file-based calls on that file; nothing is copied to the
+ * host and u, v, alpha, the word counter and the shard states are left untouched.
+ * A name is read as the file's reader reads it (at most 50 characters, upper-cased); a name holding ' ' or '\n' cannot
+ * survive the file and is W2B_EINVAL, as are a NULL ctx or words and a k outside 1..W2B_MAX_TOPK.  W2B_ESTATE before
+ * w2b_init_tables / w2b_checkpoint_load.  The call runs on the context's device: it first waits for the context's
+ * stream, and returns with nothing left running and every temporary device buffer freed (a failed allocation is
+ * W2B_ECUDA; the context stays usable).  A 1-bit or 2-bit context evaluated with bitlevel 0 or its own level is scored
+ * in the bit domain (st->packed = 1, as for its packed file), without an fp32 table; every other case forms the fp32
+ * table on the device.  gpu_ms includes the kernel that builds the table or the bit planes from u and v. */
+int w2b_ctx_compute_accuracy(w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+                             const char *questions_file, w2b_accuracy *acc, char *report, int64_t report_cap);
+int w2b_ctx_analogy_answers(w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+                            const char *questions_file, int32_t *answers, int64_t answers_cap, int64_t *n_questions);
+int w2b_ctx_analogy_topk(w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+                         const char *questions_file, int k, int32_t *ids, float *scores, int64_t cap_queries,
+                         int64_t *n_queries, w2b_topk_stats *st);
+int w2b_ctx_nearest(w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold, const char *words_file,
+                    int k, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries, w2b_topk_stats *st);
+
 /* Multi-GPU replica averaging (SURVEY §8(e)); G=1 contexts never touch NCCL. */
 int w2b_device_ptrs(w2b_ctx *ctx, void **u, void **v, int64_t *elems);
 int w2b_nccl_unique_id(void *id128);                                    /* ncclGetUniqueId */

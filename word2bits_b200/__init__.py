@@ -256,6 +256,65 @@ class Trainer:
         check(lib.w2b_checkpoint_load(self.h, path.encode(), C.byref(n)))
         return n.value
 
+    # -- evaluation of the tables as they stand (quantize(u + v), what export() returns), no file in between
+    def _names(self, names):
+        """The row names as a C array (kept alive with the returned object)."""
+        if names is None:
+            if self.corpus is None:
+                raise ValueError("a Trainer built without a corpus needs the row names")
+            names = self.corpus.words()
+        enc = [n if isinstance(n, bytes) else n.encode("latin1") for n in names]
+        if len(enc) != self.V:
+            raise ValueError("%d names for %d rows" % (len(enc), self.V))
+        return (C.c_char_p * len(enc))(*enc)
+
+    def compute_accuracy(self, questions_file, names=None, bitlevel=0, threshold=0):
+        """compute_accuracy on this context's tables: (report text, dict of counters), exactly what the module-level
+        compute_accuracy returns on the file export() would be written to (-binary 1), names = the row names."""
+        words = self._names(names)
+        acc = _lib.Accuracy()
+        buf = C.create_string_buffer(1 << 20)
+        check(lib.w2b_ctx_compute_accuracy(self.h, words, int(bitlevel), int(threshold), questions_file.encode(),
+                                           C.byref(acc), buf, len(buf)))
+        return buf.value.decode("latin1"), {k: getattr(acc, k) for k, _ in acc._fields_}
+
+    def analogy_answers(self, questions_file, names=None, bitlevel=0, threshold=0):
+        """analogy_answers on this context's tables (int32 numpy array, one entry per question)."""
+        words = self._names(names)
+        ans = np.empty(os.path.getsize(questions_file) // 4 + 1, np.int32)
+        n = C.c_int64()
+        check(lib.w2b_ctx_analogy_answers(self.h, words, int(bitlevel), int(threshold), questions_file.encode(),
+                                          ptr(ans), len(ans), C.byref(n)))
+        return ans[: n.value].copy()
+
+    def _topk(self, fn, input_file, k, names, bitlevel, threshold):
+        words = self._names(names)
+        args = (self.h, words, int(bitlevel), int(threshold), input_file.encode() if input_file else None, int(k))
+        n = C.c_int64()
+        check(fn(*args, None, None, 0, C.byref(n), None))
+        ids = np.empty((max(n.value, 1), max(int(k), 1)), np.int32)
+        scores = np.empty(ids.shape, np.float32)
+        st = _lib.TopkStats()
+        check(fn(*args, ptr(ids), ptr(scores), max(n.value, 1), C.byref(n), C.byref(st)))
+        return ids[: n.value].copy(), scores[: n.value].copy(), st.as_dict()
+
+    def analogy_topk(self, questions_file, k, names=None, bitlevel=0, threshold=0):
+        """analogy_topk on this context's tables: (ids int32 [n, k], scores float32 [n, k], stats)."""
+        return self._topk(lib.w2b_ctx_analogy_topk, questions_file, k, names, bitlevel, threshold)
+
+    def nearest(self, query_words_or_file, k, names=None, bitlevel=0, threshold=0):
+        """nearest on this context's tables: query_words_or_file is a list of words or the path of a file of
+        whitespace-separated words.  Returns (ids int32 [n, k], scores float32 [n, k], stats)."""
+        if isinstance(query_words_or_file, (list, tuple)):
+            import tempfile
+            with tempfile.NamedTemporaryFile("w", suffix=".txt", delete=False) as f:
+                f.write("\n".join(query_words_or_file) + "\n")
+            try:
+                return self._topk(lib.w2b_ctx_nearest, f.name, k, names, bitlevel, threshold)
+            finally:
+                os.unlink(f.name)
+        return self._topk(lib.w2b_ctx_nearest, query_words_or_file, k, names, bitlevel, threshold)
+
     # -- multi-GPU
     def device_ptrs(self):
         u, v, n = C.c_void_p(), C.c_void_p(), C.c_int64()

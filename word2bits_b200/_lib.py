@@ -91,6 +91,7 @@ EXPORTS = [
     "w2b_analogy_answers", "w2b_eval_filter_scores",
     "w2b_compute_accuracy_packed", "w2b_analogy_answers_packed", "w2b_eval_packed_scores",
     "w2b_analogy_topk", "w2b_nearest",
+    "w2b_ctx_compute_accuracy", "w2b_ctx_analogy_answers", "w2b_ctx_analogy_topk", "w2b_ctx_nearest",
     "w2b_host_unigram_bounds", "w2b_host_exptable", "w2b_host_keep_thresholds", "w2b_host_lcg_tables", "w2b_warp_plan_query", "w2b_host_gather_slices",
     "w2b_kernel_query",
 ]
@@ -134,6 +135,10 @@ lib.w2b_analogy_topk.argtypes = [C.c_char_p, C.c_int, _i64, C.c_char_p, C.c_int,
                                  _P(TopkStats)]
 lib.w2b_nearest.argtypes = [C.c_char_p, C.c_int, _i64, C.c_char_p, C.c_int, C.c_int, _vp, _vp, _i64, _P(_i64),
                             _P(TopkStats)]
+lib.w2b_ctx_compute_accuracy.argtypes = [_vp, _vp, C.c_int, _i64, C.c_char_p, _P(Accuracy), C.c_char_p, _i64]
+lib.w2b_ctx_analogy_answers.argtypes = [_vp, _vp, C.c_int, _i64, C.c_char_p, _vp, _i64, _P(_i64)]
+lib.w2b_ctx_analogy_topk.argtypes = [_vp, _vp, C.c_int, _i64, C.c_char_p, C.c_int, _vp, _vp, _i64, _P(_i64), _P(TopkStats)]
+lib.w2b_ctx_nearest.argtypes = [_vp, _vp, C.c_int, _i64, C.c_char_p, C.c_int, _vp, _vp, _i64, _P(_i64), _P(TopkStats)]
 lib.w2b_host_unigram_bounds.argtypes = [_vp, _i64, _vp]
 lib.w2b_host_exptable.argtypes = [_vp]
 lib.w2b_host_keep_thresholds.argtypes = [_vp, _i64, _i64, _f, _vp]

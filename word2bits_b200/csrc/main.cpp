@@ -12,6 +12,9 @@
 //   -binary 2    packed output: bitlevel bits per value (bitlevel 1 and 2), see w2b_write_packed.
 //   -checkpoint F  write a resumable checkpoint (fp32 u, v, alpha, word counter) to F after every epoch.
 //   -resume F      continue from checkpoint F at the epoch it was written after.
+//   -eval FILE     after every epoch, evaluate the model as it stands on the analogy questions of FILE (the
+//                  evaluator on the context's own tables, bitlevel 0) and print the last two lines of the report
+//                  compute_accuracy prints on the epoch's vector file; -eval-threshold N = its <threshold> (default 0).
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -113,6 +116,18 @@ int main(int argc, char **argv) {
   if ((i = arg_pos("-sync-mode", argc, argv)) > 0) sync_mode = atoi(argv[i + 1]);
   if (ngpus < 1) ngpus = 1;
   if (sync_every < 1) sync_every = 1;
+  std::string eval_file;
+  long long eval_threshold = 0;
+  if ((i = arg_pos("-eval", argc, argv)) > 0) eval_file = argv[i + 1];
+  if ((i = arg_pos("-eval-threshold", argc, argv)) > 0) eval_threshold = atoll(argv[i + 1]);
+  if (!eval_file.empty()) {  // checked now rather than after an epoch of training
+    FILE *f = fopen(eval_file.c_str(), "rb");
+    if (!f) {
+      printf("ERROR: questions file %s not found!\n", eval_file.c_str());
+      exit(1);
+    }
+    fclose(f);
+  }
 
   printf("Starting training using file %s\n", train_file.c_str());  // :523
   w2b_corpus *corpus = nullptr;
@@ -207,6 +222,12 @@ int main(int argc, char **argv) {
     if (G > 1 && w2b_nccl_init(ctx, uid, rank, G)) die("w2b_nccl_init");  // (after the tables hold their starting point)
     std::vector<float> buf;
     if (rank == 0) buf.resize((size_t)V * layer1_size);
+    std::vector<const char *> names;  // row names for -eval
+    std::vector<char> report;
+    if (rank == 0 && !eval_file.empty()) {
+      for (long long w = 0; w < V; ++w) names.push_back(w2b_corpus_word(corpus, w));
+      report.resize(1 << 20);  // compute_accuracy's report buffer
+    }
     for (int iteration = (int)first_epoch; iteration < iter; iteration++) {
       if (rank == 0) {
         printf("Starting epoch: %d\n", iteration);  // :533
@@ -251,6 +272,19 @@ int main(int argc, char **argv) {
       }
       if (rank == 0) {
         printf("Epoch Loss: %lf\n", epoch_loss);  // :539
+        if (!eval_file.empty()) {  // (several GPUs: the epoch's last exchange has made the replicas equal)
+          w2b_accuracy acc;
+          if (w2b_ctx_compute_accuracy(ctx, names.data(), 0, eval_threshold, eval_file.c_str(), &acc, report.data(),
+                                       (int64_t)report.size()))
+            die("w2b_ctx_compute_accuracy");
+          // the report's last two lines: "Total accuracy: ..." and "Questions seen / total: ..."
+          const std::string text(report.data());
+          size_t from = text.size();
+          int newlines = 0;
+          while (from > 0 && !(text[from - 1] == '\n' && ++newlines == 3)) --from;
+          fputs(text.c_str() + from, stdout);
+          fflush(stdout);
+        }
         if (!ckpt_file.empty() && w2b_checkpoint_save(ctx, ckpt_file.c_str(), iteration + 1)) die("w2b_checkpoint_save");
         if (classes == 0 && save_every_epoch) {  // :540-557
           char name[4200];

@@ -1297,6 +1297,20 @@ extern "C" int w2b_export(w2b_ctx *c, float *out) {
   return W2B_OK;
 }
 
+int w2b_ctx_tables_of(w2b_ctx *c, w2b_ctx_tables *out) {
+  NEED(c);
+  if (!c->have_tables) { w2b_set_error("init_tables or checkpoint_load first"); return W2B_ESTATE; }
+  out->u = c->d_u;
+  out->v = c->d_v;
+  out->V = c->cfg.vocab_size;
+  out->D = c->cfg.layer1_size;
+  out->pitch = c->plan.pitch;
+  out->bitlevel = c->cfg.bitlevel;
+  out->device = c->cfg.device;
+  out->stream = c->stream;
+  return W2B_OK;
+}
+
 extern "C" int w2b_quantize(w2b_ctx *c, const float *in, float *out, int64_t n, int bitlevel) {
   NEED(c);
   if (n <= 0) return W2B_OK;

@@ -100,6 +100,20 @@ __global__ void eval_query_kernel(const float *M, const int *q3, float *Q, long 
   Q[q * Dp + a] = __fadd_rn(__fsub_rn(M[b2 * Dp + a], M[b1 * Dp + a]), M[b3 * Dp + a]);
 }
 
+// The fp32 table of a training context: row r of M (Dp floats apart, padding columns left as they are) =
+// quantize(u + v) of row r with export_kernel's arithmetic, i.e. the row w2b_export returns and -binary 1 writes.
+// One warp per row; u and v rows are `pitch` floats apart and their padding columns are not read.
+__global__ void eval_ctx_table_kernel(const float *u, const float *v, long long pitch, float *M, long long words,
+                                      long long D, long long Dp, int bits) {
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= words) return;
+  QParams qp;
+  qp.bits = bits;
+  qp.seg = (bits >= 4) ? exp2f((float)(bits - 1)) : 1.f;
+  for (long long a = lane; a < D; a += 32) M[row * Dp + a] = quant<9>(__fadd_rn(u[row * pitch + a], v[row * pitch + a]), qp);
+}
+
 // eps of the tensor-core filter per question, a bound on |approx - ref| where ref is the score in the reference's fp32
 // order and approx the tensor core's.  With u = 2^-24 and sum|v_a m_a| <= |vec| |m| (Cauchy-Schwarz), |m| = 1:
 //   operands: TF32 keeps 10 explicit mantissa bits of each (the rest is dropped), so a product is off by at most
@@ -231,6 +245,32 @@ std::string upper(std::string s) {
   return s;
 }
 
+// The table an evaluation reads, with the names of its rows: a vector file read into host memory, or a training
+// context's u and v, which stay on the device (the scoring behind it is the same for both).
+struct Table {
+  std::vector<std::string> names;
+  long long words = 0, size = 0;
+  std::vector<float> M;              // word2vec-binary file: words x size floats
+  std::vector<uint8_t> rows;         // packed file: words packed rows
+  int bits = 0;                      // 1 or 2: scored in the bit domain (a packed file, or the context's own levels)
+  const w2b_ctx_tables *ctx = nullptr;
+};
+
+// The fp32 table on the device, rows Dp floats apart and zero padded: upload_fp32 before the timed kernels (a file's
+// table is copied), build_fp32 as the first of them (a context's table is formed from u and v).
+int upload_fp32(const Table &t, float *dM, long long Dp) {
+  CKE(cudaMemset(dM, 0, (size_t)t.words * Dp * sizeof(float)));
+  if (!t.ctx)
+    CKE(cudaMemcpy2D(dM, Dp * sizeof(float), t.M.data(), t.size * sizeof(float), t.size * sizeof(float), t.words,
+                     cudaMemcpyHostToDevice));
+  return W2B_OK;
+}
+void build_fp32(const Table &t, float *dM, long long Dp) {
+  if (t.ctx)
+    eval_ctx_table_kernel<<<(unsigned)((t.words + 7) / 8), 256>>>(t.ctx->u, t.ctx->v, t.ctx->pitch, dM, t.words, t.size,
+                                                                 Dp, t.ctx->bitlevel);
+}
+
 }  // namespace
 
 // Reads the word2vec-binary file exactly like :85-111 (names up to the first ' ', '\n' skipped,
@@ -269,9 +309,19 @@ static int read_vectors(const char *path, long long threshold, std::vector<std::
   return W2B_OK;
 }
 
-static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t threshold,
-                                 const char *questions_file, int device, w2b_accuracy *acc, char *report,
-                                 int64_t report_cap, int32_t *answers, int64_t answers_cap, int64_t *n_questions);
+static int compute_accuracy_impl(const Table &t, int bitlevel, const char *questions_file, int device, w2b_accuracy *acc,
+                                 char *report, int64_t report_cap, int32_t *answers, int64_t answers_cap,
+                                 int64_t *n_questions);
+// a word2vec-binary file's table, then the evaluation
+static int compute_accuracy_file(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file,
+                                 int device, w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers,
+                                 int64_t answers_cap, int64_t *n_questions) {
+  Table t;
+  const int rc = read_vectors(vectors_file, threshold, t.names, t.M, t.words, t.size);
+  if (rc) return rc;
+  return compute_accuracy_impl(t, bitlevel, questions_file, device, acc, report, report_cap, answers, answers_cap,
+                               n_questions);
+}
 // nothing is thrown across the C ABI (std::bad_alloc on a huge vocabulary, ...)
 template <class F> static int no_throw(const char *who, F &&f) {
   try {
@@ -290,7 +340,7 @@ extern "C" int w2b_compute_accuracy(const char *vectors_file, int bitlevel, int6
   if (!vectors_file) { w2b_set_error("w2b_compute_accuracy: null vectors_file"); return W2B_EINVAL; }
   if (report && report_cap > 0) report[0] = 0;
   return no_throw("w2b_compute_accuracy", [&] {
-    return compute_accuracy_impl(vectors_file, bitlevel, threshold, questions_file, device, acc, report, report_cap,
+    return compute_accuracy_file(vectors_file, bitlevel, threshold, questions_file, device, acc, report, report_cap,
                                  nullptr, 0, nullptr);
   });
 }
@@ -298,7 +348,7 @@ extern "C" int w2b_analogy_answers(const char *vectors_file, int bitlevel, int64
                                    int device, int32_t *answers, int64_t answers_cap, int64_t *n_questions) {
   if (!vectors_file) { w2b_set_error("w2b_analogy_answers: null vectors_file"); return W2B_EINVAL; }
   return no_throw("w2b_analogy_answers", [&] {
-    return compute_accuracy_impl(vectors_file, bitlevel, threshold, questions_file, device, nullptr, nullptr, 0, answers,
+    return compute_accuracy_file(vectors_file, bitlevel, threshold, questions_file, device, nullptr, nullptr, 0, answers,
                                  answers_cap, n_questions);
   });
 }
@@ -364,16 +414,13 @@ static void write_report(const Questions &qs, const std::vector<std::string> &na
                          w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers, int64_t answers_cap,
                          int64_t *n_questions);
 
-static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t threshold,
-                                 const char *questions_file, int device, w2b_accuracy *acc, char *report,
-                                 int64_t report_cap, int32_t *answers, int64_t answers_cap, int64_t *n_questions) {
-  std::vector<std::string> names;
-  std::vector<float> M;
-  long long words = 0, size = 0;
-  int rc = read_vectors(vectors_file, threshold, names, M, words, size);
-  if (rc) return rc;
+static int compute_accuracy_impl(const Table &t, int bitlevel, const char *questions_file, int device, w2b_accuracy *acc,
+                                 char *report, int64_t report_cap, int32_t *answers, int64_t answers_cap,
+                                 int64_t *n_questions) {
+  const std::vector<std::string> &names = t.names;
+  const long long words = t.words, size = t.size;
   Questions qs;
-  rc = parse_questions(questions_file, names, qs);
+  int rc = parse_questions(questions_file, names, qs);
   if (rc) return rc;
   const std::vector<int> &q3 = qs.q3;
   const long long nq = (long long)q3.size() / 3;
@@ -406,9 +453,8 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
     float *dM = bM.as<float>(), *dQ = bQ.as<float>();
     int *dq3 = bq3.as<int>();
     unsigned long long *dbest = bbest.as<unsigned long long>(), *dcnt = bcnt.as<unsigned long long>();
-    CKE(cudaMemset(dM, 0, (size_t)words * Dp * sizeof(float)));
+    if ((rc = upload_fp32(t, dM, Dp))) return rc;
     CKE(cudaMemset(dQ, 0, (size_t)nq * Dp * sizeof(float)));
-    CKE(cudaMemcpy2D(dM, Dp * sizeof(float), M.data(), size * sizeof(float), size * sizeof(float), words, cudaMemcpyHostToDevice));
     CKE(cudaMemcpy(dq3, q3.data(), q3.size() * sizeof(int), cudaMemcpyHostToDevice));
     CKE(cudaMemset(dbest, 0, nq * sizeof(unsigned long long)));
     CKE(cudaMemset(bgmax.p, 0, nq * sizeof(unsigned)));
@@ -417,6 +463,7 @@ static int compute_accuracy_impl(const char *vectors_file, int bitlevel, int64_t
     CKE(cudaEventCreate(&e0.e));
     CKE(cudaEventCreate(&e1.e));
     CKE(cudaEventRecord(e0.e));
+    build_fp32(t, dM, Dp);
     eval_normalize_kernel<<<(unsigned)((words + 7) / 8), 256>>>(dM, words, size, Dp, bitlevel);
     eval_query_kernel<<<(unsigned)((nq * size + 255) / 256), 256>>>(dM, dq3, dQ, nq, size, Dp);
     bool need_simt = simt;
@@ -594,10 +641,12 @@ struct BitsState {
   long long V = 0, nbytes = 0, nq = 0, chunk = 0;
   int D = 0, Wp = 0, W = 0;
   unsigned long long cand_cap = 0;
+  const w2b_ctx_tables *ctx = nullptr;  // set: the planes come from the context's u + v (rows is then NULL)
 };
 
-// Device buffers of one run: rows = V packed rows nbytes apart, qid = the W distinct query words, q3w = per question
-// its three rows of G (indices into qid), q3 = per question the three vocabulary ids that cannot be its answer.
+// Device buffers of one run: rows = V packed rows nbytes apart (NULL: the planes come from st.ctx), qid = the W distinct
+// query words, q3w = per question its three rows of G (indices into qid), q3 = per question the three vocabulary ids
+// that cannot be its answer.
 int bits_upload(BitsState &st, const uint8_t *rows, long long V, int D, int bits, const int *qid, int W, const int *q3w,
                 const int *q3, long long nq, unsigned long long cand_cap) {
   st.V = V; st.D = D; st.W = W; st.nq = nq; st.cand_cap = cand_cap;
@@ -605,7 +654,7 @@ int bits_upload(BitsState &st, const uint8_t *rows, long long V, int D, int bits
   st.Wp = ((D + 31) / 32 + 3) & ~3;
   const long long vround = (V + bits::CT - 1) / bits::CT * bits::CT;
   st.chunk = std::min<long long>(vround, std::max<long long>(bits::CT, (long long)(kGramChunkBytes / 4 / W) / bits::CT * bits::CT));
-  CKE(st.rows.alloc((size_t)V * st.nbytes));
+  if (rows) CKE(st.rows.alloc((size_t)V * st.nbytes));
   CKE(st.sign.alloc((size_t)V * st.Wp * 4));
   if (bits == 2) CKE(st.mag.alloc((size_t)V * st.Wp * 4));
   CKE(st.len.alloc(V * 4));
@@ -620,10 +669,12 @@ int bits_upload(BitsState &st, const uint8_t *rows, long long V, int D, int bits
   CKE(st.cnt.alloc(2 * sizeof(unsigned long long)));
   CKE(st.cand.alloc(cand_cap * sizeof(tc::Candidate)));
   CKE(st.G.alloc((size_t)W * st.chunk * 4));
-  HostPin pin;
-  CKE(cudaHostRegister((void *)rows, (size_t)V * st.nbytes, cudaHostRegisterDefault));
-  pin.p = (void *)rows;
-  CKE(cudaMemcpy(st.rows.p, rows, (size_t)V * st.nbytes, cudaMemcpyHostToDevice));
+  if (rows) {
+    HostPin pin;
+    CKE(cudaHostRegister((void *)rows, (size_t)V * st.nbytes, cudaHostRegisterDefault));
+    pin.p = (void *)rows;
+    CKE(cudaMemcpy(st.rows.p, rows, (size_t)V * st.nbytes, cudaMemcpyHostToDevice));
+  }
   CKE(cudaMemcpy(st.qid.p, qid, (size_t)W * 4, cudaMemcpyHostToDevice));
   CKE(cudaMemcpy(st.q3.p, q3, (size_t)nq * 12, cudaMemcpyHostToDevice));
   CKE(cudaMemcpy(st.q3w.p, q3w, (size_t)nq * 12, cudaMemcpyHostToDevice));
@@ -634,9 +685,14 @@ int bits_upload(BitsState &st, const uint8_t *rows, long long V, int D, int bits
 
 // planes + row lengths, then eps and the scale factors of every question
 template <int BITS> int bits_planes(BitsState &st) {
-  bits::eval_bits_planes_kernel<BITS><<<(unsigned)((st.V + 7) / 8), 256>>>(
-      st.rows.as<uint8_t>(), st.V, st.D, st.nbytes, st.Wp, st.sign.as<unsigned>(), st.mag.as<unsigned>(), st.len.as<float>(),
-      st.ilen.as<float>(), st.hpop.as<int>());
+  if (st.ctx)
+    bits::eval_ctx_planes_kernel<BITS><<<(unsigned)((st.V + 7) / 8), 256>>>(
+        st.ctx->u, st.ctx->v, st.ctx->pitch, st.V, st.D, st.Wp, st.sign.as<unsigned>(), st.mag.as<unsigned>(),
+        st.len.as<float>(), st.ilen.as<float>(), st.hpop.as<int>());
+  else
+    bits::eval_bits_planes_kernel<BITS><<<(unsigned)((st.V + 7) / 8), 256>>>(
+        st.rows.as<uint8_t>(), st.V, st.D, st.nbytes, st.Wp, st.sign.as<unsigned>(), st.mag.as<unsigned>(),
+        st.len.as<float>(), st.ilen.as<float>(), st.hpop.as<int>());
   bits::eval_bits_qeps_kernel<BITS><<<(unsigned)((st.nq + 7) / 8), 256>>>(
       st.sign.as<unsigned>(), st.mag.as<unsigned>(), st.len.as<float>(), st.qid.as<int>(), st.q3w.as<int>(), st.qk.as<float>(),
       st.qeps.as<float>(), st.nq, st.D, st.Wp);
@@ -751,17 +807,14 @@ void distinct_words(const std::vector<int> &q3, std::vector<int> &qid, std::vect
   }
 }
 
-int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, const char *questions_file, int device,
-                                 w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers,
-                                 int64_t answers_cap, int64_t *n_questions) {
-  std::vector<std::string> names;
-  std::vector<uint8_t> rows;
-  long long words = 0, size = 0;
-  int file_bits = 0;
-  int rc = read_packed(packed_file, threshold, names, rows, words, size, file_bits);
-  if (rc) return rc;
+// a packed table (t.bits = 1 or 2: a packed file, or a context on the bit-domain route)
+int compute_accuracy_packed_impl(const Table &t, const char *questions_file, int device, w2b_accuracy *acc, char *report,
+                                 int64_t report_cap, int32_t *answers, int64_t answers_cap, int64_t *n_questions) {
+  const std::vector<std::string> &names = t.names;
+  const long long words = t.words, size = t.size;
+  const int file_bits = t.bits;
   Questions qs;
-  rc = parse_questions(questions_file, names, qs);
+  int rc = parse_questions(questions_file, names, qs);
   if (rc) return rc;
   const long long nq = (long long)qs.q3.size() / 3;
   std::vector<int> qid, q3w;
@@ -780,8 +833,9 @@ int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, con
     const char *dbg = getenv("W2B_EVAL_SIMT");
     const bool simt = dbg && atoi(dbg) != 0;
     BitsState st;
+    st.ctx = t.ctx;
     DevBuf bbest;
-    rc = bits_upload(st, rows.data(), words, (int)size, file_bits, qid.data(), (int)qid.size(), q3w.data(), qs.q3.data(), nq,
+    rc = bits_upload(st, t.ctx ? nullptr : t.rows.data(), words, (int)size, file_bits, qid.data(), (int)qid.size(), q3w.data(), qs.q3.data(), nq,
                      (unsigned long long)nq * 1024ull);  // the cap of the tensor-core filter's list
     if (rc) return rc;
     CKE(bbest.alloc(nq * sizeof(unsigned long long)));
@@ -807,6 +861,16 @@ int compute_accuracy_packed_impl(const char *packed_file, int64_t threshold, con
   return W2B_OK;
 }
 
+int compute_accuracy_packed_file(const char *packed_file, int64_t threshold, const char *questions_file, int device,
+                                 w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers,
+                                 int64_t answers_cap, int64_t *n_questions) {
+  Table t;
+  const int rc = read_packed(packed_file, threshold, t.names, t.rows, t.words, t.size, t.bits);
+  if (rc) return rc;
+  return compute_accuracy_packed_impl(t, questions_file, device, acc, report, report_cap, answers, answers_cap,
+                                      n_questions);
+}
+
 }  // namespace
 
 extern "C" int w2b_compute_accuracy_packed(const char *packed_file, int64_t threshold, const char *questions_file,
@@ -814,7 +878,7 @@ extern "C" int w2b_compute_accuracy_packed(const char *packed_file, int64_t thre
   if (!packed_file) { w2b_set_error("w2b_compute_accuracy_packed: null packed_file"); return W2B_EINVAL; }
   if (report && report_cap > 0) report[0] = 0;
   return no_throw("w2b_compute_accuracy_packed", [&] {
-    return compute_accuracy_packed_impl(packed_file, threshold, questions_file, device, acc, report, report_cap, nullptr,
+    return compute_accuracy_packed_file(packed_file, threshold, questions_file, device, acc, report, report_cap, nullptr,
                                         0, nullptr);
   });
 }
@@ -825,7 +889,7 @@ extern "C" int w2b_analogy_answers_packed(const char *packed_file, int64_t thres
     return W2B_EINVAL;
   }
   return no_throw("w2b_analogy_answers_packed", [&] {
-    return compute_accuracy_packed_impl(packed_file, threshold, questions_file, device, nullptr, nullptr, 0, answers,
+    return compute_accuracy_packed_file(packed_file, threshold, questions_file, device, nullptr, nullptr, 0, answers,
                                         answers_cap, n_questions);
   });
 }
@@ -1124,26 +1188,16 @@ int packed_bits_of(const char *path) {
   return (int)bits;
 }
 
-int topk_impl(const char *vectors_file, int bitlevel, int64_t threshold, bool nearest, const char *input, int k,
-              int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries, w2b_topk_stats *stats) {
+// t: the table (names only matter when cap_queries > 0: counting the queries needs no vectors); packed = t.bits, the
+// level of a packed file or of a context on the bit-domain route, 0 for an fp32 table.
+int topk_impl(const Table &t, int packed, int bitlevel, bool nearest, const char *input, int k, int device, int32_t *ids,
+              float *scores, int64_t cap_queries, int64_t *n_queries, w2b_topk_stats *stats) {
   w2b_topk_stats s;
   memset(&s, 0, sizeof s);
-  const int packed = packed_bits_of(vectors_file);
-  if (packed && bitlevel != 0 && bitlevel != packed) {
-    w2b_set_error("%s holds %d-bit vectors: bitlevel must be %d or 0", vectors_file, packed, packed);
-    return W2B_EINVAL;
-  }
-  std::vector<std::string> names;
-  std::vector<float> M;
-  std::vector<uint8_t> rows;
-  long long words = 0, size = 0;
-  int file_bits = 0;
+  const std::vector<std::string> &names = t.names;
+  const long long words = t.words, size = t.size;
+  const int file_bits = packed;
   int rc = W2B_OK;
-  if (cap_queries > 0) {  // (counting the queries needs no vectors: no word is then in the vocabulary)
-    rc = packed ? read_packed(vectors_file, threshold, names, rows, words, size, file_bits)
-                : read_vectors(vectors_file, threshold, names, M, words, size);
-    if (rc) return rc;
-  }
   // per output row (file order): the query it is, or -1 (a word is not in the vocabulary)
   std::vector<int> q3, row_q;
   if (nearest) {
@@ -1186,12 +1240,11 @@ int topk_impl(const char *vectors_file, int bitlevel, int64_t threshold, bool ne
     if (!packed) {
       DevEvent e0, e1;
       CKE(bM.alloc((size_t)words * Dp * sizeof(float)));
-      CKE(cudaMemset(bM.p, 0, (size_t)words * Dp * sizeof(float)));
-      CKE(cudaMemcpy2D(bM.p, Dp * sizeof(float), M.data(), size * sizeof(float), size * sizeof(float), words,
-                       cudaMemcpyHostToDevice));
+      if ((rc = upload_fp32(t, bM.as<float>(), Dp))) return rc;
       CKE(cudaEventCreate(&e0.e));
       CKE(cudaEventCreate(&e1.e));
       CKE(cudaEventRecord(e0.e));
+      build_fp32(t, bM.as<float>(), Dp);
       eval_normalize_kernel<<<(unsigned)((words + 7) / 8), 256>>>(bM.as<float>(), words, size, Dp, bitlevel);
       CKE(cudaEventRecord(e1.e));
       CKE(cudaEventSynchronize(e1.e));
@@ -1209,9 +1262,10 @@ int topk_impl(const char *vectors_file, int bitlevel, int64_t threshold, bool ne
         rc = topk_fp32(bM.as<float>(), words, size, sub, simt, b, s, &s.gpu_ms);
       } else {
         BitsState st;
+        st.ctx = t.ctx;
         std::vector<int> qid, q3w;
         distinct_words(sub, qid, q3w);
-        if ((rc = bits_upload(st, rows.data(), words, (int)size, file_bits, qid.data(), (int)qid.size(), q3w.data(),
+        if ((rc = bits_upload(st, t.ctx ? nullptr : t.rows.data(), words, (int)size, file_bits, qid.data(), (int)qid.size(), q3w.data(),
                               sub.data(), nb, 1)))  // (its arg-max candidate list is not used)
           return rc;
         rc = file_bits == 1 ? topk_packed<1>(st, simt, b, s, &s.gpu_ms) : topk_packed<2>(st, simt, b, s, &s.gpu_ms);
@@ -1236,6 +1290,22 @@ int topk_impl(const char *vectors_file, int bitlevel, int64_t threshold, bool ne
   return W2B_OK;
 }
 
+int topk_file(const char *vectors_file, int bitlevel, int64_t threshold, bool nearest, const char *input, int k,
+              int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries, w2b_topk_stats *stats) {
+  const int packed = packed_bits_of(vectors_file);
+  if (packed && bitlevel != 0 && bitlevel != packed) {
+    w2b_set_error("%s holds %d-bit vectors: bitlevel must be %d or 0", vectors_file, packed, packed);
+    return W2B_EINVAL;
+  }
+  Table t;
+  if (cap_queries > 0) {  // (counting the queries needs no vectors: no word is then in the vocabulary)
+    const int rc = packed ? read_packed(vectors_file, threshold, t.names, t.rows, t.words, t.size, t.bits)
+                          : read_vectors(vectors_file, threshold, t.names, t.M, t.words, t.size);
+    if (rc) return rc;
+  }
+  return topk_impl(t, packed, bitlevel, nearest, input, k, device, ids, scores, cap_queries, n_queries, stats);
+}
+
 int topk_args(const char *who, const char *vectors_file, int k, const int32_t *ids, const float *scores,
               int64_t cap_queries) {
   if (!vectors_file || k < 1 || k > W2B_MAX_TOPK || cap_queries < 0 || (cap_queries > 0 && (!ids || !scores))) {
@@ -1253,7 +1323,7 @@ extern "C" int w2b_analogy_topk(const char *vectors_file, int bitlevel, int64_t 
                                 w2b_topk_stats *st) {
   if (int rc = topk_args("w2b_analogy_topk", vectors_file, k, ids, scores, cap_queries)) return rc;
   return no_throw("w2b_analogy_topk", [&] {
-    return topk_impl(vectors_file, bitlevel, threshold, false, questions_file, k, device, ids, scores, cap_queries,
+    return topk_file(vectors_file, bitlevel, threshold, false, questions_file, k, device, ids, scores, cap_queries,
                      n_queries, st);
   });
 }
@@ -1263,7 +1333,128 @@ extern "C" int w2b_nearest(const char *vectors_file, int bitlevel, int64_t thres
                            w2b_topk_stats *st) {
   if (int rc = topk_args("w2b_nearest", vectors_file, k, ids, scores, cap_queries)) return rc;
   return no_throw("w2b_nearest", [&] {
-    return topk_impl(vectors_file, bitlevel, threshold, true, words_file, k, device, ids, scores, cap_queries, n_queries,
+    return topk_file(vectors_file, bitlevel, threshold, true, words_file, k, device, ids, scores, cap_queries, n_queries,
                      st);
+  });
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// The evaluator on a training context's own tables (w2b_ctx_*): the table is quantize(u + v), formed on the device from
+// u and v, with words[i] the name of row i.  The route follows from what the context holds: a 1-bit or 2-bit context
+// evaluated at its own level (bitlevel 0 or the same) is scored in the bit domain from planes built straight from u and
+// v (eval_ctx_planes_kernel), as its packed file would be; every other case fills the fp32 table that -binary 1 would
+// write (eval_ctx_table_kernel) and runs the fp32 pipeline.  Either way nothing is copied to the host and u, v, alpha,
+// the word counter and the shard states are only read.
+namespace {
+
+// names as read_vectors reads them from the written file (at most 50 characters, upper-cased); the context's stream
+// is drained first, since training may still be running on it
+int ctx_table(const char *who, w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+              w2b_ctx_tables &ct, Table &t) {
+  int rc = w2b_ctx_tables_of(ctx, &ct);
+  if (rc) return rc;
+  t.words = (threshold > 0 && ct.V > threshold) ? threshold : ct.V;
+  t.size = ct.D;
+  t.names.resize(t.words);
+  for (long long b = 0; b < t.words; ++b) {
+    const char *w = words[b];
+    if (!w || strpbrk(w, " \n")) {  // a name the file round trip cannot carry
+      w2b_set_error("%s: the name of row %lld %s", who, b, w ? "contains ' ' or '\\n'" : "is NULL");
+      return W2B_EINVAL;
+    }
+    std::string n;
+    for (const char *p = w; *p && n.size() < 50; ++p) n.push_back(*p);
+    t.names[b] = upper(n);
+  }
+  t.ctx = &ct;
+  t.bits = ((ct.bitlevel == 1 || ct.bitlevel == 2) && (bitlevel == 0 || bitlevel == ct.bitlevel)) ? ct.bitlevel : 0;
+  CKE(cudaSetDevice(ct.device));
+  CKE(cudaStreamSynchronize((cudaStream_t)ct.stream));
+  return W2B_OK;
+}
+
+int ctx_topk_args(const char *who, int k, const int32_t *ids, const float *scores, int64_t cap_queries) {
+  if (k < 1 || k > W2B_MAX_TOPK || cap_queries < 0 || (cap_queries > 0 && (!ids || !scores))) {
+    w2b_set_error("%s: bad arguments (k = %d: 1 <= k <= %d, ids and scores for %lld rows)", who, k, W2B_MAX_TOPK,
+                  (long long)cap_queries);
+    return W2B_EINVAL;
+  }
+  return W2B_OK;
+}
+
+template <class F> int ctx_call(const char *who, w2b_ctx *ctx, const char *const *words, F &&f) {
+  if (!ctx || !words) {
+    w2b_set_error("%s: null %s", who, ctx ? "words" : "ctx");
+    return W2B_EINVAL;
+  }
+  const int rc = no_throw(who, f);
+  if (rc) (void)cudaGetLastError();  // e.g. a failed allocation: not reported again by the context's next call
+  return rc;
+}
+
+int ctx_accuracy(const char *who, w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+                 const char *questions_file, w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers,
+                 int64_t answers_cap, int64_t *n_questions) {
+  w2b_ctx_tables ct;
+  Table t;
+  const int rc = ctx_table(who, ctx, words, bitlevel, threshold, ct, t);
+  if (rc) return rc;
+  return t.bits ? compute_accuracy_packed_impl(t, questions_file, ct.device, acc, report, report_cap, answers,
+                                               answers_cap, n_questions)
+                : compute_accuracy_impl(t, bitlevel, questions_file, ct.device, acc, report, report_cap, answers,
+                                        answers_cap, n_questions);
+}
+
+int ctx_topk(const char *who, w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold, bool nearest,
+             const char *input, int k, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries,
+             w2b_topk_stats *st) {
+  w2b_ctx_tables ct;
+  Table t;
+  const int rc = ctx_table(who, ctx, words, bitlevel, threshold, ct, t);
+  if (rc) return rc;
+  return topk_impl(t, t.bits, bitlevel, nearest, input, k, ct.device, ids, scores, cap_queries, n_queries, st);
+}
+
+}  // namespace
+
+extern "C" int w2b_ctx_compute_accuracy(w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+                                        const char *questions_file, w2b_accuracy *acc, char *report, int64_t report_cap) {
+  if (report && report_cap > 0) report[0] = 0;
+  return ctx_call("w2b_ctx_compute_accuracy", ctx, words, [&] {
+    return ctx_accuracy("w2b_ctx_compute_accuracy", ctx, words, bitlevel, threshold, questions_file, acc, report,
+                        report_cap, nullptr, 0, nullptr);
+  });
+}
+
+extern "C" int w2b_ctx_analogy_answers(w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+                                       const char *questions_file, int32_t *answers, int64_t answers_cap,
+                                       int64_t *n_questions) {
+  if (!answers && answers_cap > 0) {
+    w2b_set_error("w2b_ctx_analogy_answers: null answers");
+    return W2B_EINVAL;
+  }
+  return ctx_call("w2b_ctx_analogy_answers", ctx, words, [&] {
+    return ctx_accuracy("w2b_ctx_analogy_answers", ctx, words, bitlevel, threshold, questions_file, nullptr, nullptr, 0,
+                        answers, answers_cap, n_questions);
+  });
+}
+
+extern "C" int w2b_ctx_analogy_topk(w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+                                    const char *questions_file, int k, int32_t *ids, float *scores, int64_t cap_queries,
+                                    int64_t *n_queries, w2b_topk_stats *st) {
+  if (int rc = ctx_topk_args("w2b_ctx_analogy_topk", k, ids, scores, cap_queries)) return rc;
+  return ctx_call("w2b_ctx_analogy_topk", ctx, words, [&] {
+    return ctx_topk("w2b_ctx_analogy_topk", ctx, words, bitlevel, threshold, false, questions_file, k, ids, scores,
+                    cap_queries, n_queries, st);
+  });
+}
+
+extern "C" int w2b_ctx_nearest(w2b_ctx *ctx, const char *const *words, int bitlevel, int64_t threshold,
+                               const char *words_file, int k, int32_t *ids, float *scores, int64_t cap_queries,
+                               int64_t *n_queries, w2b_topk_stats *st) {
+  if (int rc = ctx_topk_args("w2b_ctx_nearest", k, ids, scores, cap_queries)) return rc;
+  return ctx_call("w2b_ctx_nearest", ctx, words, [&] {
+    return ctx_topk("w2b_ctx_nearest", ctx, words, bitlevel, threshold, true, words_file, k, ids, scores, cap_queries,
+                    n_queries, st);
   });
 }

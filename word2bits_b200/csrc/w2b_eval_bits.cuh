@@ -6,7 +6,8 @@
 // (driven from w2b_eval.cu):
 //   planes   eval_bits_planes_kernel: the file's rows -> a sign plane and a magnitude plane of uint32 words on a
 //            16-byte row pitch (padding bits 0), popc of the magnitude plane, and the row's fp32 length summed in
-//            the order eval_normalize_kernel uses (the reference's build order);
+//            the order eval_normalize_kernel uses (the reference's build order); eval_ctx_planes_kernel builds the
+//            same planes from a training context's u + v (the evaluator on a context's own tables);
 //   Gram     eval_bits_gram_kernel: G[w][c] = integer dot of distinct query word w and vocabulary word c, a chunk of
 //            the vocabulary at a time;
 //   combine  eval_bits_combine_kernel: approx(q, c) = (G[w2][c]/len2 - G[w1][c]/len1 + G[w3][c]/len3) unit / len_c, the
@@ -44,9 +45,31 @@ __device__ __forceinline__ unsigned even_bits(unsigned long long x) {
   return (unsigned)x;
 }
 
+// What both plane kernels derive from a row's plane words, which they feed in order k = 0, 1, ...: popc of the
+// magnitude plane and the row's fp32 length, every value's square added in index order as every lane of
+// eval_normalize_kernel does (the squares of the first 4*floor(D/4) values rounded on their own and added one at a
+// time, the last D mod 4 fused).  The two kernels differ only in where the bits come from.
+template <int BITS> struct RowLength {
+  float s = 0.f;
+  int ph = 0;
+  __device__ __forceinline__ void add(unsigned n, unsigned h, int k, int D) {
+    const int valid = min(32, max(0, D - 32 * k)), D4 = D & ~3;
+    ph += __popc(h);
+    for (int j = 0; j < valid; ++j) {
+      const float q = level<BITS>((n >> j) & 1u, (h >> j) & 1u);
+      s = (32 * k + j < D4) ? __fadd_rn(s, __fmul_rn(q, q)) : __fmaf_rn(q, q, s);
+    }
+  }
+  __device__ __forceinline__ void store(long long row, float *len, float *ilen, int *hpop) const {
+    const float l = __fsqrt_rn(s);
+    len[row] = l;
+    ilen[row] = (float)(1.0 / (double)l);  // one rounding of the exact reciprocal
+    hpop[row] = ph;
+  }
+};
+
 // One warp per row.  Every lane assembles plane word k from the row's bytes (the same addresses in all lanes: one
-// broadcast load each) and adds the 32 squares in index order, as every lane of eval_normalize_kernel does: the
-// squares of the first 4*floor(D/4) values rounded on their own and added one at a time, the last D mod 4 fused.
+// broadcast load each) and adds the 32 squares in index order (RowLength).
 // rows are nbytes apart (the file's row, no alignment); Wp = plane words per row, a multiple of 4.
 template <int BITS>
 __global__ void eval_bits_planes_kernel(const uint8_t *rows, long long V, int D, long long nbytes, int Wp, unsigned *sign,
@@ -55,9 +78,7 @@ __global__ void eval_bits_planes_kernel(const uint8_t *rows, long long V, int D,
   const int lane = threadIdx.x & 31;
   if (row >= V) return;
   const uint8_t *r = rows + row * nbytes;
-  const int D4 = D & ~3;
-  float s = 0.f;
-  int ph = 0;
+  RowLength<BITS> rl;
   for (int k = 0; k < Wp; ++k) {
     unsigned long long raw = 0;
     const long long b0 = (long long)k * 4 * BITS;
@@ -72,18 +93,44 @@ __global__ void eval_bits_planes_kernel(const uint8_t *rows, long long V, int D,
       sign[row * Wp + k] = n;
       if (BITS == 2) mag[row * Wp + k] = h;
     }
-    ph += __popc(h);
-    for (int j = 0; j < valid; ++j) {
-      const float q = level<BITS>((n >> j) & 1u, (h >> j) & 1u);
-      s = (32 * k + j < D4) ? __fadd_rn(s, __fmul_rn(q, q)) : __fmaf_rn(q, q, s);
+    rl.add(n, h, k, D);
+  }
+  if (lane == 0) rl.store(row, len, ilen, hpop);
+}
+
+// The same planes straight from a training context's tables: value a of row `row` is quantize(u + v) exactly as
+// export_kernel forms it (the row w2b_export returns), and its codes are the ones w2b_write_packed writes for that
+// value (sign: < 0; magnitude: |x| > 0.5).  Lane l reads column 32 k + l of u and v (rows `pitch` floats apart,
+// padding columns not read) and the warp's ballots are plane word k, padding bits 0: bit for bit what
+// eval_bits_planes_kernel derives from the packed file of w2b_export's output.
+template <int BITS>
+__global__ void eval_ctx_planes_kernel(const float *u, const float *v, long long pitch, long long V, int D, int Wp,
+                                       unsigned *sign, unsigned *mag, float *len, float *ilen, int *hpop) {
+  const long long row = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= V) return;  // (the whole warp: the ballots below see every lane)
+  QParams qp;
+  qp.bits = BITS;
+  qp.seg = 1.f;
+  const float *ur = u + row * pitch, *vr = v + row * pitch;
+  RowLength<BITS> rl;
+  for (int k = 0; k < Wp; ++k) {
+    const int a = 32 * k + lane;
+    bool neg = false, big = false;
+    if (a < D) {
+      const float x = quant<9>(__fadd_rn(ur[a], vr[a]), qp);
+      neg = x < 0.f;
+      big = fabsf(x) > 0.5f;
     }
+    const unsigned n = __ballot_sync(kFull, neg);
+    const unsigned h = (BITS == 2) ? __ballot_sync(kFull, big) : 0u;
+    if (lane == 0) {
+      sign[row * Wp + k] = n;
+      if (BITS == 2) mag[row * Wp + k] = h;
+    }
+    rl.add(n, h, k, D);
   }
-  if (lane == 0) {
-    const float l = __fsqrt_rn(s);
-    len[row] = l;
-    ilen[row] = (float)(1.0 / (double)l);  // one rounding of the exact reciprocal
-    hpop[row] = ph;
-  }
+  if (lane == 0) rl.store(row, len, ilen, hpop);
 }
 
 // G[w * ldg + (c - c0)] for w in [0, W), c in [c0, c0 + nc): the exact integer dot of rows qid[w] and c.

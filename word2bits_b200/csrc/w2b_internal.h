@@ -41,6 +41,17 @@ int w2b_packed_open(const char *path, w2b_packed_file *pf);
 // The next word: at most name_cap - 1 characters of its name (NUL-terminated; name may be NULL) and its nbytes
 // packed bytes.  W2B_EIO when the file ends inside the row.
 int w2b_packed_next(w2b_packed_file *pf, char *name, int name_cap, uint8_t *row);
+// What the evaluator reads of a training context (w2b_ctx_compute_accuracy and friends): the fp32 master tables u
+// and v, V rows of `pitch` floats of which the first D are the row (the rest is padding), the training bit level,
+// the context's device and its stream (a cudaStream_t).  W2B_ESTATE before w2b_init_tables / w2b_checkpoint_load.
+struct w2b_ctx;
+struct w2b_ctx_tables {
+  const float *u = nullptr, *v = nullptr;
+  int64_t V = 0, D = 0, pitch = 0;
+  int bitlevel = 0, device = 0;
+  void *stream = nullptr;
+};
+int w2b_ctx_tables_of(w2b_ctx *ctx, w2b_ctx_tables *out);
 // InitUnigramTable (src/word2bits.cpp:112-128) in boundary form: start[i] = first table
 // slot owned by word i, start[V] = 1e8.  Same libm pow() and the same double arithmetic
 // as the reference loop, so expanding it reproduces the 1e8-entry table bit for bit.
