@@ -135,7 +135,8 @@ typedef struct {
 typedef struct {
   int32_t center, b, cw, ntargets;
   int32_t targets[64];
-  float alpha;
+  float alpha; /* the learning rate the position trains with (w2b_trace: as one shard alone would see it, from the
+                  configured alpha and a counter of its own; w2b_train_step_traced: the shared value the shard read) */
 } w2b_trace_rec;
 
 const char *w2b_last_error(void);
@@ -203,6 +204,10 @@ int w2b_train_epoch(w2b_ctx *ctx, double *loss, w2b_step_stats *stats);
 /* Parity hooks */
 int w2b_trace(w2b_ctx *ctx, int shard, int64_t max_iterations, w2b_trace_rec *out, int64_t cap,
               int64_t *n_out); /* draws only; does not touch u/v or shard state */
+/* Exactly w2b_train_step, and local shard i's draw records of the step, in order, at recs[i * cap_per_shard ...];
+ * n_per_shard[i] = how many it made (may exceed the cap: only the first cap_per_shard are stored). */
+int w2b_train_step_traced(w2b_ctx *ctx, int64_t words_per_shard, w2b_step_stats *stats, w2b_trace_rec *recs,
+                          int64_t cap_per_shard, int64_t *n_per_shard);
 int w2b_strict_prefix(w2b_ctx *ctx, int shard, int64_t max_iterations, double *loss); /* strict mode: first k iterations of a shard */
 int w2b_apply_position(w2b_ctx *ctx, const int32_t *context_ids, int cw, const int32_t *targets,
                        int ntargets, float *f_out); /* Appendix-A steps 5-7 for explicit ids */

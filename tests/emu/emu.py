@@ -46,10 +46,12 @@ class EmuError(RuntimeError):
 
 def train_epoch_warp(corpus, table, u, v, *, size, window, negative, bitlevel, shards, serial=0, alpha=0.05,
                      sample=1e-3, iters=1, async_mode=1, seed=1, state=None, trace_shard=None, trace_cap=0, max_iters=-1,
-                     slots=0, fault=0, reg=0.0):
+                     slots=0, fault=0, reg=0.0, trace_train=False):
     """One pass of every shard (one 32-thread CTA after another) through the emulated warp-per-shard kernel
     (csrc/w2b_warp.cuh).  u, v are updated in place.  Returns a dict of per-shard statistics; `state` carries
-    (alpha, word_count_actual) across epochs."""
+    (alpha, word_count_actual) across epochs.  With trace_cap the kernel records every shard's draws in its own
+    region (the layout of w2b_train_step_traced): out["traces"][i] is shard i's, out["trace"] that of `trace_shard`.
+    Tracing runs draws only (trace_shard alone), unless trace_train: then every shard trains as well."""
     plan = w2b.warp_plan(size=size, window=window, negative=negative, bitlevel=bitlevel, vocab_size=corpus.vocab_size,
                          slots=slots, reg=reg)
     if not plan["warp"]:
@@ -62,8 +64,8 @@ def train_epoch_warp(corpus, table, u, v, *, size, window, negative, bitlevel, s
     wca = np.array([0 if state is None else state[1]], np.uint64)
     out = dict(loss=np.zeros(shards), words=np.zeros(shards, np.int64), n_pos=np.zeros(shards, np.int64),
                n_ctx=np.zeros(shards, np.int64), n_tgt=np.zeros(shards, np.int64), done=np.zeros(shards, np.int32))
-    trace = (_lib.TraceRec * max(trace_cap, 1))()
-    trace_n = np.zeros(1, np.uint64)
+    trace = (_lib.TraceRec * max(trace_cap * shards, 1))()
+    trace_n = np.zeros(shards, np.uint64)
     p = _lib.ptr
     pitch = (size + 3) // 4 * 4  # the device layout: rows padded to whole float4s, padding zero
     u_in, v_in = u, v
@@ -76,7 +78,7 @@ def train_epoch_warp(corpus, table, u, v, *, size, window, negative, bitlevel, s
                serial=serial,
                u=p(u), v=p(v), table=p(table), keep=p(keep), exptab=p(exptab), tokens=p(tokens), n_tokens=len(tokens),
                shard_start=p(start), shard_first=p(first), alpha=p(a), wca=p(wca), word_budget=0, max_iters=max_iters,
-               seed=seed, async_mode=async_mode, train=0 if trace_cap else 1,
+               seed=seed, async_mode=async_mode, train=0 if trace_cap and not trace_train else 1,
                loss=p(out["loss"]), words=p(out["words"]), n_pos=p(out["n_pos"]), n_ctx=p(out["n_ctx"]),
                n_tgt=p(out["n_tgt"]), done=p(out["done"]),
                trace=C.cast(trace, C.c_void_p) if trace_cap else None, trace_cap=trace_cap,
@@ -92,6 +94,10 @@ def train_epoch_warp(corpus, table, u, v, *, size, window, negative, bitlevel, s
     out["alpha"], out["wca"] = float(a[0]), int(wca[0])
     out["plan"] = plan
     if trace_cap:
-        n = int(trace_n[0])
-        out["trace"] = [(t.center, t.b, t.cw, list(t.targets[: t.ntargets]), t.alpha) for t in trace[: min(n, trace_cap)]]
+        out["traces"] = [[(t.center, t.b, t.cw, list(t.targets[: t.ntargets]), t.alpha)
+                          for t in trace[i * trace_cap: i * trace_cap + min(int(trace_n[i]), trace_cap)]]
+                         for i in range(shards)]
+        out["trace_n"] = trace_n.astype(np.int64)
+        if trace_shard is not None:
+            out["trace"] = out["traces"][trace_shard]
     return out

@@ -378,8 +378,8 @@ struct EmuRun {
   double *loss;
   int64_t *words, *n_pos, *n_ctx, *n_tgt;
   int32_t *done;
-  w2b_trace_rec *trace;
-  int64_t trace_cap;
+  w2b_trace_rec *trace;  // per shard, as w2b_train_step_traced lays it out: shard i's records at trace[i * trace_cap ..),
+  int64_t trace_cap;     // their count in trace_n[i] (num_shards entries)
   uint64_t *trace_n;
   int32_t only_shard;  // >= 0: run just this shard
   int32_t fault;       // 0; 1 / 2: injected protocol faults (negative controls, see g_fault)
@@ -442,7 +442,7 @@ static void emu_setup(const EmuRun *r, std::vector<w2b::ShardState> &shards, w2b
   p.shard_word_limit = r->train_words / r->num_shards;
   p.word_budget = r->word_budget; p.max_iters = r->max_iters; p.shard_base = 0; p.train = r->train;
   p.serial = r->serial; p.wca_scale = 1;
-  p.trace = r->trace; p.trace_cap = r->trace_cap; p.trace_n = (unsigned long long *)r->trace_n;
+  p.trace = r->trace; p.trace_cap = r->trace_cap; p.trace_n = (unsigned long long *)r->trace_n; p.trace_per_shard = 1;
 }
 
 static void emu_results(const EmuRun *r, const std::vector<w2b::ShardState> &shards) {

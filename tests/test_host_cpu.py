@@ -32,6 +32,17 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, n), n
 
 
+def test_train_step_traced_refuses_bad_arguments():
+    """Refused with W2B_EINVAL before any device is touched: no counts array, a negative cap, records missing."""
+    from word2bits_b200 import _lib
+    n = np.zeros(4, np.int64)
+    recs = ctypes.cast((_lib.TraceRec * 4)(), ctypes.c_void_p)
+    for args, msg in [((None, 1, None, recs, 1, None), "n_per_shard"), ((None, 1, None, recs, -1, _lib.ptr(n)), "cap"),
+                      ((None, 1, None, None, 1, _lib.ptr(n)), "recs"), ((None, 1, None, recs, 1, _lib.ptr(n)), "null c")]:
+        assert _lib.lib.w2b_train_step_traced(*args) == _lib.EINVAL, msg
+        assert msg in _lib.lib.w2b_last_error().decode(), (msg, _lib.lib.w2b_last_error())
+
+
 def test_no_cpu_fallback():
     import word2bits_b200 as w2b
     if _has_gpu():

@@ -15,8 +15,9 @@ bench.py times: 1584 shards at D = 800 on an H100 SXM) is replayed from the draw
     float32 add's rounding per update: every update lands exactly once;
   * rows no shard touched are bit-identical, the loss lies within the sum of the shards' loss intervals, and the
     counters equal the sums over the traces.
-No shard crosses a 10 000-word learning-rate period inside a checked step (asserted from the traces), so every
-position trains at the alpha get_state() reports before the step.
+No shard crosses a 10 000-word learning-rate period inside a checked step here (asserted from the traces), so every
+position trains at the alpha get_state() reports before the step; tests/test_shards_alpha_f64.py checks steps in which
+every shard crosses one, or reaches its end, at the alphas w2b_train_step_traced records.
 
 On the CPU a Hogwild executor built on the oracle's single-position step interleaves shards in random order, lands
 each update late and shows every read a random element-wise prefix of the other shards' landed updates; it passes the

@@ -196,6 +196,20 @@ class Trainer:
         check(lib.w2b_trace(self.h, shard, max_iterations, C.cast(recs, C.c_void_p), cap, C.byref(n)))
         return [(r.center, r.b, r.cw, list(r.targets[: r.ntargets]), r.alpha) for r in recs[: n.value]]
 
+    def train_step_traced(self, words_per_shard, cap):
+        """train_step, and every local shard's draw records of the step (at most `cap` each) in the format of trace();
+        a record's alpha is the learning rate its position trained with.  Returns (stats, [records of shard i],
+        [records shard i made, capped or not])."""
+        st = _lib.StepStats()
+        nloc = (self.cfg.shard_end or self.threads) - self.cfg.shard_begin
+        recs = (_lib.TraceRec * max(cap * nloc, 1))()
+        n = np.zeros(nloc, np.int64)
+        check(lib.w2b_train_step_traced(self.h, int(words_per_shard), C.byref(st), C.cast(recs, C.c_void_p), int(cap),
+                                        ptr(n)))
+        out = [[(r.center, r.b, r.cw, list(r.targets[: r.ntargets]), r.alpha)
+                for r in recs[i * cap: i * cap + min(int(n[i]), cap)]] for i in range(nloc)]
+        return st.as_dict(), out, n.tolist()
+
     def strict_prefix(self, shard, max_iterations):
         loss = C.c_double()
         check(lib.w2b_strict_prefix(self.h, shard, max_iterations, C.byref(loss)))

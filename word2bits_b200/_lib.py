@@ -84,7 +84,7 @@ EXPORTS = [
     "w2b_corpus_tokens", "w2b_corpus_shards", "w2b_write_vectors", "w2b_last_error", "w2b_device_count",
     "w2b_suggest_shards", "w2b_create", "w2b_destroy", "w2b_set_vocab_counts", "w2b_set_corpus",
     "w2b_init_tables", "w2b_epoch_begin", "w2b_train_step", "w2b_train_epoch", "w2b_trace",
-    "w2b_strict_prefix", "w2b_apply_position", "w2b_get_state", "w2b_set_state", "w2b_download_raw",
+    "w2b_train_step_traced", "w2b_strict_prefix", "w2b_apply_position", "w2b_get_state", "w2b_set_state", "w2b_download_raw",
     "w2b_upload_raw", "w2b_download_table", "w2b_download_exptable", "w2b_export", "w2b_quantize",
     "w2b_device_ptrs", "w2b_nccl_unique_id", "w2b_nccl_init", "w2b_sync", "w2b_sync_timed", "w2b_table_checksum", "w2b_scale_tables",
     "w2b_write_packed", "w2b_read_packed_header", "w2b_read_packed", "w2b_checkpoint_save", "w2b_checkpoint_load", "w2b_compute_accuracy",
@@ -157,6 +157,7 @@ lib.w2b_epoch_begin.argtypes = [_vp]
 lib.w2b_train_step.argtypes = [_vp, _i64, _P(StepStats)]
 lib.w2b_train_epoch.argtypes = [_vp, _P(C.c_double), _P(StepStats)]
 lib.w2b_trace.argtypes = [_vp, C.c_int, _i64, _vp, _i64, _P(_i64)]
+lib.w2b_train_step_traced.argtypes = [_vp, _i64, _P(StepStats), _vp, _i64, _vp]
 lib.w2b_strict_prefix.argtypes = [_vp, C.c_int, _i64, _P(C.c_double)]
 lib.w2b_apply_position.argtypes = [_vp, _vp, C.c_int, _vp, C.c_int, _vp]
 lib.w2b_get_state.argtypes = [_vp, _P(_f), _P(_i64)]

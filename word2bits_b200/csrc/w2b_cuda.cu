@@ -906,11 +906,30 @@ static int launch_train(w2b_ctx *c, TrainParams p, w2b_step_stats *acc) {
   return launch_finish(c, acc);
 }
 
-static int w2b_train_step_impl(w2b_ctx *c, int64_t words_per_shard, w2b_step_stats *stats);
+// Per-shard draw records of a training step (w2b_train_step_traced): device buffers that live for every launch of the
+// step, so that a shard's records continue across bounded launches and streamed slices.
+struct StepTrace {
+  w2b_trace_rec *recs;
+  int64_t cap;
+  int64_t *n;
+};
+
+static int w2b_train_step_impl(w2b_ctx *c, int64_t words_per_shard, w2b_step_stats *stats, const StepTrace *tr);
 extern "C" int w2b_train_step(w2b_ctx *c, int64_t words_per_shard, w2b_step_stats *stats) {
-  return w2b_guarded("w2b_train_step", [&] { return w2b_train_step_impl(c, words_per_shard, stats); });
+  return w2b_guarded("w2b_train_step", [&] { return w2b_train_step_impl(c, words_per_shard, stats, nullptr); });
 }
-static int w2b_train_step_impl(w2b_ctx *c, int64_t words_per_shard, w2b_step_stats *stats) {
+extern "C" int w2b_train_step_traced(w2b_ctx *c, int64_t words_per_shard, w2b_step_stats *stats,
+                                     w2b_trace_rec *recs, int64_t cap_per_shard, int64_t *n_per_shard) {
+  return w2b_guarded("w2b_train_step_traced", [&] {
+    NEED(n_per_shard);
+    if (cap_per_shard < 0) { w2b_set_error("w2b_train_step_traced: negative cap"); return W2B_EINVAL; }
+    if (cap_per_shard > 0) NEED(recs);
+    NEED(c);
+    const StepTrace tr{recs, cap_per_shard, n_per_shard};
+    return w2b_train_step_impl(c, words_per_shard, stats, &tr);
+  });
+}
+static int w2b_train_step_impl(w2b_ctx *c, int64_t words_per_shard, w2b_step_stats *stats, const StepTrace *tr) {
   NEED(c);
   if (!c->have_corpus || !c->have_tables || !c->have_counts) {
     w2b_set_error("train_step before set_vocab_counts/set_corpus/init_tables");
@@ -921,6 +940,20 @@ static int w2b_train_step_impl(w2b_ctx *c, int64_t words_per_shard, w2b_step_sta
   memset(&acc, 0, sizeof acc);
   sum_shards(c->h_shards, &before);
   TrainParams p = base_params(c);
+  DevTmp t_tr, t_cnt;
+  if (tr) {
+    if (tr->cap > ((int64_t)1 << 40) / (int64_t)sizeof(w2b_trace_rec) / std::max(c->nlocal, 1)) {
+      w2b_set_error("w2b_train_step_traced: cap_per_shard %lld too large", (long long)tr->cap);
+      return W2B_EINVAL;
+    }
+    CK(t_tr.alloc((size_t)std::max<int64_t>(tr->cap * c->nlocal, 1) * sizeof(w2b_trace_rec)));
+    CK(t_cnt.alloc(sizeof(unsigned long long) * c->nlocal));
+    CK(cudaMemsetAsync(t_cnt.p, 0, sizeof(unsigned long long) * c->nlocal, c->stream));
+    p.trace = t_tr.as<w2b_trace_rec>();
+    p.trace_cap = tr->cap;
+    p.trace_n = t_cnt.as<unsigned long long>();
+    p.trace_per_shard = 1;
+  }
   // The production kernel keeps 32-bit job and row counters per launch and the streaming path stages one slice
   // per shard in pinned memory, so a step is cut into bounded launches: 4 M words per shard per launch
   // (resident) / 1 M words per slice (streaming).  Steps up to those sizes are exactly one launch.
@@ -987,6 +1020,16 @@ static int w2b_train_step_impl(w2b_ctx *c, int64_t words_per_shard, w2b_step_sta
     CK(cudaMemcpy(&stats->alpha, c->d_alpha, sizeof(float), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(&wca, c->d_wca, sizeof wca, cudaMemcpyDeviceToHost));
     stats->word_count_actual = (int64_t)wca;
+  }
+  if (tr) {
+    std::vector<unsigned long long> n(c->nlocal);
+    CK(cudaMemcpy(n.data(), p.trace_n, sizeof(unsigned long long) * c->nlocal, cudaMemcpyDeviceToHost));
+    for (int i = 0; i < c->nlocal; ++i) {
+      tr->n[i] = (int64_t)n[i];
+      const int64_t k = std::min<int64_t>((int64_t)n[i], tr->cap);
+      if (k) CK(cudaMemcpy(tr->recs + i * tr->cap, p.trace + i * tr->cap, k * sizeof(w2b_trace_rec),
+                           cudaMemcpyDeviceToHost));
+    }
   }
   return W2B_OK;
 }

@@ -77,9 +77,11 @@ struct TrainParams {
   int serial;                   // warp kernel: 1 = position p+1 is fetched after every update of p completed
   int wca_scale;                // multi-GPU: local words stand for wca_scale x as many globally
   int *sen;                     // warp kernel: global sentence buffers (kMaxS ints per local shard + 1) when they do not fit shared memory
-  w2b_trace_rec *trace;
-  long long trace_cap;
+  w2b_trace_rec *trace;         // parity hooks (nullptr in production): draw records, at most trace_cap per region,
+  long long trace_cap;          // and their count (which may exceed the cap)
   unsigned long long *trace_n;
+  int trace_per_shard;          // 1: local shard i's region is trace[i * trace_cap ..), its count trace_n[i]
+                                // (w2b_train_step_traced); 0: every CTA uses region 0 (w2b_trace: one CTA)
 };
 
 // ------------------------------------------------------------------------- scalar bits
@@ -568,10 +570,11 @@ __device__ __forceinline__ void train_shards(TrainParams p) {
       if (lane == 0) d->alpha = *(volatile float *)p.alpha;
     }
     __syncthreads();
-    if (tid == 0 && p.trace) {
-      unsigned long long slot = (*p.trace_n)++;
+    if (tid == 0 && p.trace) {  // parity hook: one record per window draw
+      const long long shard = (long long)(p.shard_base + (int)blockIdx.x) * p.trace_per_shard;  // its region
+      unsigned long long slot = p.trace_n[shard]++;
       if ((long long)slot < p.trace_cap) {
-        w2b_trace_rec *t = p.trace + slot;
+        w2b_trace_rec *t = p.trace + shard * p.trace_cap + slot;
         t->center = d->center; t->b = d->b; t->cw = d->cw; t->ntargets = d->nt; t->alpha = d->alpha;
         for (int k = 0; k < d->nt; ++k) t->targets[k] = d->tg[k];
       }

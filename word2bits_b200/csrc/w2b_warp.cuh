@@ -270,9 +270,10 @@ __device__ inline int warp_next_position(const TrainParams &p, const ShardState 
     __syncwarp();                  // the queue entries are visible to every lane
     if (p.trace) {  // parity hook: one record per window draw, exactly what the oracle's trace holds
       if (lane == 0) {
-        const unsigned long long k = (*p.trace_n)++;
+        const long long shard = (long long)(p.shard_base + (int)blockIdx.x) * p.trace_per_shard;  // its region
+        const unsigned long long k = p.trace_n[shard]++;
         if ((long long)k < p.trace_cap) {
-          w2b_trace_rec *tr = p.trace + k;
+          w2b_trace_rec *tr = p.trace + shard * p.trace_cap + k;
           tr->center = center; tr->b = b; tr->cw = cw; tr->ntargets = nt; tr->alpha = S.alpha_c;
           for (int i = 0; i < nt; ++i) tr->targets[i] = jobq[(qtail + cw + i) & qmask] & kJobIdMask;
         }
