@@ -66,6 +66,28 @@ int w2b_write_packed(const char *path, const w2b_corpus *c, const float *vectors
 int w2b_read_packed_header(const char *path, int64_t *V, int64_t *D, int *bitlevel);
 int w2b_read_packed(const char *path, float *vectors /* V*D */, char *words /* V*max_word */, int max_word);
 
+/* Vector file kinds, and the one rule that tells them apart.  A first line of three integers is a packed file.  A first
+ * line of two integers "V D" is a text file (-binary 0: per word "<word> " then D values "%lf " then "\n") when (a) the
+ * byte right after the 4 D bytes that follow the first name's ' ' is not '\n' and (b) the bytes from that ' ' to the
+ * first '\n' are exactly D tokens of the grammar of w2b_host_parse_floats.  Every other file is word2vec binary (every
+ * binary file has '\n' after its first row's 4 D bytes; a "%lf " value takes at least 9 bytes).
+ * *V = the header's word count (at most threshold when threshold > 0), *D = its size, *bits = a packed file's bit level
+ * (else 0).  W2B_EIO only when the file cannot be opened. */
+#define W2B_VECTORS_BINARY 0
+#define W2B_VECTORS_TEXT 1
+#define W2B_VECTORS_PACKED 2
+int w2b_vector_file_info(const char *path, int64_t threshold, int *kind, int64_t *V, int64_t *D, int *bits);
+/* The names of the first V rows (w2b_vector_file_info) of any vector file as the evaluator compares them: up to the
+ * first ' ', '\n' skipped, at most 50 characters, upper-cased; name i at names[i*max_word], NUL-terminated (cut to
+ * max_word - 1 characters).  *n = the rows read. */
+int w2b_vector_names(const char *path, int64_t threshold, char *names /* V*max_word */, int max_word, int64_t *n);
+/* A text vector file parsed on the GPU `device`: vectors = V x D floats (V, D from w2b_vector_file_info), each value
+ * the float strtof returns for its token; words as w2b_read_packed writes them.  The file is streamed through the
+ * device in chunks; no V x D array or whole text is held on the host beyond `vectors`.  W2B_EIO names the row and token
+ * of a row with too few or too many values or a token outside the grammar. */
+int w2b_read_text_vectors(const char *path, int device, float *vectors /* V*D */, char *words /* V*max_word */,
+                          int max_word);
+
 /* Host-side arithmetic of the path, callable (and tested) without a GPU.  The device path uses exactly
  * these functions for what it uploads: unigram boundaries (InitUnigramTable :112-128 in boundary form:
  * start[i] = first of the 1e8 table slots owned by word i, start[V] = 1e8), expTable (:614-618, same libm
@@ -76,6 +98,11 @@ int w2b_host_unigram_bounds(const int64_t *cn, int64_t V, int32_t *start /* V+1 
 int w2b_host_exptable(float *out /* 1000 */);
 int w2b_host_keep_thresholds(const int64_t *cn, int64_t V, int64_t train_words, float sample, float *out /* V */);
 int w2b_host_lcg_tables(uint64_t *ja /*65*/, uint64_t *jc /*65*/, uint64_t *pa /*64*/, uint64_t *pc /*64*/);
+/* Decimal text to float32 exactly as glibc strtof rounds it (to nearest, ties to even, subnormals, +-inf past
+ * FLT_MAX, +-0 below half the smallest subnormal), with the routine the GPU text reader runs.  Tokens are separated by
+ * white space; a token is [+-]?(d+[.d*]|.d+)([eE][+-]?d+)? or, signed or not and in any case, nan, inf or infinity.
+ * out[0..*n) = the values; W2B_EIO names a token outside the grammar, W2B_EINVAL more than cap tokens. */
+int w2b_host_parse_floats(const char *text, int64_t n_bytes, float *out, int64_t cap, int64_t *n);
 
 /* The host half of a streaming step (w2b_set_corpus resident = 0): the next L tokens of every unfinished shard are
  * gathered into one pinned staging buffer (slice i at stage[i*L]) by a few host threads before the single H2D copy.

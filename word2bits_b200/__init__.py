@@ -15,7 +15,7 @@ from ._lib import MODE_FAST, MODE_STRICT, TABLE_SIZE, W2BError, check, lib, ptr
 __all__ = ["Corpus", "Trainer", "W2BError", "MODE_FAST", "MODE_STRICT", "device_count", "read_packed", "nccl_unique_id",
            "compute_accuracy", "analogy_answers", "eval_filter_scores", "compute_accuracy_packed", "analogy_answers_packed",
            "eval_packed_scores", "host_unigram_bounds", "host_exptable", "host_keep_thresholds", "host_lcg_tables", "warp_plan",
-           "analogy_topk", "nearest"]
+           "analogy_topk", "nearest", "host_parse_floats", "vector_file_info", "read_text_vectors"]
 
 
 def device_count():
@@ -380,8 +380,42 @@ def read_packed(path, max_word=64):
     return words, vec, b.value
 
 
+def host_parse_floats(text):
+    """The float32 values of the white-space separated tokens of `text` (bytes or str), each exactly what glibc strtof
+    returns for it, converted on the host by the routine the GPU text reader runs.  A token outside the grammar
+    [+-]?(d+[.d*]|.d+)([eE][+-]?d+)? (or nan, inf, infinity, signed or not, in any case) raises W2BError."""
+    if isinstance(text, str):
+        text = text.encode("latin1")
+    out = np.empty(max(len(text) // 2 + 1, 1), np.float32)  # a token and its separator take at least 2 bytes
+    n = C.c_int64()
+    check(lib.w2b_host_parse_floats(text, len(text), ptr(out), len(out), C.byref(n)))
+    return out[: n.value].copy()
+
+
+def vector_file_info(path, threshold=0):
+    """(kind, V, D, bits) of a vector file: kind "binary" (word2vec binary), "text" (-binary 0) or "packed"
+    (-binary 2), V its words (at most threshold when threshold > 0), D their size, bits a packed file's bit level."""
+    kind, V, D, bits = C.c_int(), C.c_int64(), C.c_int64(), C.c_int()
+    check(lib.w2b_vector_file_info(path.encode(), int(threshold), C.byref(kind), C.byref(V), C.byref(D), C.byref(bits)))
+    return ("binary", "text", "packed")[kind.value], V.value, D.value, bits.value
+
+
+def read_text_vectors(path, device=0, max_word=64):
+    """(words, vectors) of a text vector file (-binary 0, Corpus.write_vectors(binary=0)), parsed on the GPU: vectors
+    is V x D float32, each value what strtof returns for its token; words as written (cut to max_word - 1 bytes)."""
+    kind, V, D, _ = vector_file_info(path)
+    if kind != "text":
+        raise W2BError(_lib.EIO, "%s is not a text vector file" % path)
+    vec = np.empty((V, D), np.float32)
+    names = np.zeros((max(V, 1), max_word), np.uint8)
+    check(lib.w2b_read_text_vectors(path.encode(), int(device), ptr(vec), ptr(names), max_word))
+    words = [bytes(r[: list(r).index(0)] if 0 in r else r).decode("latin1") for r in names[:V]]
+    return words, vec
+
+
 def compute_accuracy(vectors_file, questions_file, bitlevel=0, threshold=0, device=0):
-    """GPU port of the reference's compute_accuracy: returns (report text, dict of counters)."""
+    """GPU port of the reference's compute_accuracy: returns (report text, dict of counters).  A word2vec-binary or
+    text (-binary 0, parsed on the GPU) vector file."""
     acc = _lib.Accuracy()
     buf = C.create_string_buffer(1 << 20)
     check(lib.w2b_compute_accuracy(vectors_file.encode(), int(bitlevel), int(threshold), questions_file.encode(),
@@ -463,7 +497,7 @@ def analogy_topk(vectors_file, questions_file, k, bitlevel=0, threshold=0, devic
     """The reference's top-N list at N = k for every question of questions_file, in file order: (ids int32 [n, k],
     scores float32 [n, k], stats).  Row i holds the k words of largest fp32 score > 0 (not the question's own words),
     best first, the smaller index first on equal scores; -1 (score 0) pads a short list and fills the row of a question
-    with a word not in the vocabulary.  Word2vec-binary or packed vector file (bitlevel then 0 or the file's)."""
+    with a word not in the vocabulary.  Word2vec-binary, text or packed vector file (bitlevel then 0 or the file's)."""
     return _topk(lib.w2b_analogy_topk, vectors_file, questions_file, k, bitlevel, threshold, device)
 
 

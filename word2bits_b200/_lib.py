@@ -10,6 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libw2b.so")
 
 OK, EINVAL, ECUDA, EIO, ESTATE, ENCCL, ENOMEM = range(7)
+VECTORS_BINARY, VECTORS_TEXT, VECTORS_PACKED = range(3)
 TABLE_SIZE = 100_000_000
 MODE_FAST, MODE_STRICT = 0, 1
 
@@ -93,7 +94,7 @@ EXPORTS = [
     "w2b_analogy_topk", "w2b_nearest",
     "w2b_ctx_compute_accuracy", "w2b_ctx_analogy_answers", "w2b_ctx_analogy_topk", "w2b_ctx_nearest",
     "w2b_host_unigram_bounds", "w2b_host_exptable", "w2b_host_keep_thresholds", "w2b_host_lcg_tables", "w2b_warp_plan_query", "w2b_host_gather_slices",
-    "w2b_kernel_query",
+    "w2b_kernel_query", "w2b_host_parse_floats", "w2b_vector_file_info", "w2b_vector_names", "w2b_read_text_vectors",
 ]
 
 if not os.path.exists(LIB_PATH):
@@ -123,6 +124,10 @@ lib.w2b_write_vectors.argtypes = [C.c_char_p, _vp, _vp, _i64, _i64, C.c_int]
 lib.w2b_write_packed.argtypes = [C.c_char_p, _vp, _vp, _i64, _i64, C.c_int]
 lib.w2b_read_packed_header.argtypes = [C.c_char_p, _P(_i64), _P(_i64), _P(C.c_int)]
 lib.w2b_read_packed.argtypes = [C.c_char_p, _vp, _vp, C.c_int]
+lib.w2b_host_parse_floats.argtypes = [C.c_char_p, _i64, _vp, _i64, _P(_i64)]
+lib.w2b_vector_file_info.argtypes = [C.c_char_p, _i64, _P(C.c_int), _P(_i64), _P(_i64), _P(C.c_int)]
+lib.w2b_vector_names.argtypes = [C.c_char_p, _i64, _vp, C.c_int, _P(_i64)]
+lib.w2b_read_text_vectors.argtypes = [C.c_char_p, C.c_int, _vp, _vp, C.c_int]
 lib.w2b_checkpoint_save.argtypes = [_vp, C.c_char_p, _i64]
 lib.w2b_checkpoint_load.argtypes = [_vp, C.c_char_p, _P(_i64)]
 lib.w2b_compute_accuracy.argtypes = [C.c_char_p, C.c_int, _i64, C.c_char_p, C.c_int, _P(Accuracy), C.c_char_p, _i64]

@@ -1,6 +1,7 @@
 // nearest — the nearest word vectors of every word read from stdin, on the GPU (w2b_nearest).
 //   ./nearest <FILE> [k=40] [bitlevel] [threshold] < words.txt
-// FILE is a word2vec-binary vector file or a packed one (`word2bits -binary 2`).  Per query word it prints
+// FILE is a word2vec-binary vector file, a text one (`word2bits -binary 0`, parsed on the GPU) or a packed one
+// (`word2bits -binary 2`).  Per query word it prints
 // "<WORD>:" and then up to k lines "<rank>\t<WORD>\t<score>", or "<WORD>: not in vocabulary".
 #include <ctype.h>
 #include <stdio.h>
@@ -15,32 +16,19 @@
 
 // the names as the evaluator compares them: up to the first ' ', '\n' skipped, at most 50 characters, upper-cased
 static bool read_names(const char *path, long long threshold, std::vector<std::string> &names) {
-  FILE *f = fopen(path, "rb");
-  if (!f) return false;
-  long long words = 0, size = 0, bits = 0;
-  char line[128], extra;
-  const bool packed = fgets(line, sizeof line, f) && sscanf(line, "%lld %lld %lld %c", &words, &size, &bits, &extra) == 3;
-  if (!packed && sscanf(line, "%lld %lld", &words, &size) != 2) { fclose(f); return false; }
-  if (threshold > 0 && words > threshold) words = threshold;
-  const long long row = packed ? (size * bits + 7) / 8 + 1 : size * 4;  // a packed row ends with '\n'
-  for (long long b = 0; b < words; ++b) {
-    std::string w;
-    for (;;) {
-      const int ch = fgetc(f);
-      if (ch == EOF || ch == ' ') break;
-      if (ch != '\n' && w.size() < 50) w.push_back((char)toupper(ch));
-    }
-    names.push_back(w);
-    if (fseek(f, row, SEEK_CUR)) break;
-  }
-  fclose(f);
+  int kind, bits;
+  int64_t V, D, n = 0;
+  if (w2b_vector_file_info(path, threshold, &kind, &V, &D, &bits) || V < 0) return false;
+  std::vector<char> buf((size_t)(V > 0 ? V : 1) * 51);
+  if (w2b_vector_names(path, threshold, buf.data(), 51, &n)) return false;
+  for (int64_t i = 0; i < n; ++i) names.push_back(&buf[(size_t)i * 51]);
   return true;
 }
 
 int main(int argc, char **argv) {
   if (argc < 2) {
     printf("Usage: ./nearest <FILE> [k=40] [bitlevel] [threshold] < words.txt\nwhere FILE contains word projections "
-           "(word2vec binary or packed), k is the length of every list (1..%d), bitlevel re-quantises an fp32 file "
+           "(word2vec binary, text or packed), k is the length of every list (1..%d), bitlevel re-quantises an fp32 file "
            "as compute_accuracy does, and threshold restricts the vocabulary to its first words (0 = off)\n",
            W2B_MAX_TOPK);
     return 0;

@@ -245,23 +245,32 @@ std::string upper(std::string s) {
   return s;
 }
 
-// The table an evaluation reads, with the names of its rows: a vector file read into host memory, or a training
-// context's u and v, which stay on the device (the scoring behind it is the same for both).
+// The table an evaluation reads, with the names of its rows: a binary or packed vector file read into host memory, a
+// text vector file parsed on the device, or a training context's u and v, which stay on the device (the scoring behind
+// it is the same for all).
 struct Table {
   std::vector<std::string> names;
   long long words = 0, size = 0;
   std::vector<float> M;              // word2vec-binary file: words x size floats
   std::vector<uint8_t> rows;         // packed file: words packed rows
+  DevBuf text;                       // text file: the fp32 table on the device (rows Dp floats apart, zero padded)
   int bits = 0;                      // 1 or 2: scored in the bit domain (a packed file, or the context's own levels)
   const w2b_ctx_tables *ctx = nullptr;
 };
 
-// The fp32 table on the device, rows Dp floats apart and zero padded: upload_fp32 before the timed kernels (a file's
-// table is copied), build_fp32 as the first of them (a context's table is formed from u and v).
-int upload_fp32(const Table &t, float *dM, long long Dp) {
-  CKE(cudaMemset(dM, 0, (size_t)t.words * Dp * sizeof(float)));
+// The fp32 table on the device, rows Dp floats apart and zero padded: upload_fp32 before the timed kernels (a binary
+// file's table is copied into bM; a text file's was parsed into place when the file was read), build_fp32 as the first
+// of them (a context's table is formed from u and v).  *dM = the table.
+int upload_fp32(const Table &t, DevBuf &bM, long long Dp, float **dM) {
+  if (t.text.p) {
+    *dM = t.text.as<float>();
+    return W2B_OK;
+  }
+  CKE(bM.alloc((size_t)t.words * Dp * sizeof(float)));
+  *dM = bM.as<float>();
+  CKE(cudaMemset(*dM, 0, (size_t)t.words * Dp * sizeof(float)));
   if (!t.ctx)
-    CKE(cudaMemcpy2D(dM, Dp * sizeof(float), t.M.data(), t.size * sizeof(float), t.size * sizeof(float), t.words,
+    CKE(cudaMemcpy2D(*dM, Dp * sizeof(float), t.M.data(), t.size * sizeof(float), t.size * sizeof(float), t.words,
                      cudaMemcpyHostToDevice));
   return W2B_OK;
 }
@@ -309,15 +318,56 @@ static int read_vectors(const char *path, long long threshold, std::vector<std::
   return W2B_OK;
 }
 
+// The kind of a vector file (w2b_vector_file_info); a file that cannot be opened is left to its reader to report.
+static int vector_kind(const char *path, int *bits) {
+  int kind = W2B_VECTORS_BINARY;
+  int64_t V, D;
+  *bits = 0;
+  if (w2b_vector_file_info(path, 0, &kind, &V, &D, bits)) kind = W2B_VECTORS_BINARY;
+  return kind;
+}
+
+// A text vector file (w2b_text.cu): the first `threshold` rows (all when threshold <= 0) parsed on the device into
+// t.text, names as read_vectors reads them.
+static int read_text(const char *path, int64_t threshold, int device, Table &t) {
+  int kind, bits;
+  int64_t V, D;
+  int rc = w2b_vector_file_info(path, threshold, &kind, &V, &D, &bits);
+  if (rc) return rc;
+  if (V < 1 || V > 0x7fffffffLL || D > (1LL << 20) || V > (1LL << 40) / D) {
+    w2b_set_error("bad header: %lld words of size %lld", (long long)V, (long long)D);
+    return W2B_EIO;
+  }
+  int ndev = 0;
+  if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0 || device < 0 || device >= ndev) {
+    w2b_set_error("no CUDA device %d: the evaluator has no CPU fallback", device);
+    return W2B_ECUDA;
+  }
+  CKE(cudaSetDevice(device));
+  const long long Dp = (D + tc::BK - 1) / tc::BK * tc::BK;
+  CKE(t.text.alloc((size_t)V * Dp * sizeof(float)));
+  CKE(cudaMemset(t.text.p, 0, (size_t)V * Dp * sizeof(float)));
+  std::vector<std::string> raw;
+  if ((rc = w2b_text_parse(path, V, D, t.text.as<float>(), Dp, raw))) return rc;
+  t.names.resize(V);
+  for (int64_t b = 0; b < V; ++b) t.names[b] = upper(raw[b].substr(0, 50));
+  t.words = V;
+  t.size = D;
+  return W2B_OK;
+}
+
 static int compute_accuracy_impl(const Table &t, int bitlevel, const char *questions_file, int device, w2b_accuracy *acc,
                                  char *report, int64_t report_cap, int32_t *answers, int64_t answers_cap,
                                  int64_t *n_questions);
-// a word2vec-binary file's table, then the evaluation
+// a word2vec-binary or text file's table, then the evaluation
 static int compute_accuracy_file(const char *vectors_file, int bitlevel, int64_t threshold, const char *questions_file,
                                  int device, w2b_accuracy *acc, char *report, int64_t report_cap, int32_t *answers,
                                  int64_t answers_cap, int64_t *n_questions) {
   Table t;
-  const int rc = read_vectors(vectors_file, threshold, t.names, t.M, t.words, t.size);
+  int bits;
+  const int rc = vector_kind(vectors_file, &bits) == W2B_VECTORS_TEXT
+                     ? read_text(vectors_file, threshold, device, t)
+                     : read_vectors(vectors_file, threshold, t.names, t.M, t.words, t.size);
   if (rc) return rc;
   return compute_accuracy_impl(t, bitlevel, questions_file, device, acc, report, report_cap, answers, answers_cap,
                                n_questions);
@@ -442,7 +492,6 @@ static int compute_accuracy_impl(const Table &t, int bitlevel, const char *quest
     const bool simt = dbg && atoi(dbg) != 0;
     DevBuf bM, bQ, bq3, bbest, bgmax, bcand, bqeps, bcnt;
     const unsigned long long cand_cap = (unsigned long long)nq * 1024ull;  // measured: tens to hundreds per question
-    CKE(bM.alloc((size_t)words * Dp * sizeof(float)));
     CKE(bQ.alloc((size_t)nq * Dp * sizeof(float)));
     CKE(bq3.alloc(q3.size() * sizeof(int)));
     CKE(bbest.alloc(nq * sizeof(unsigned long long)));
@@ -450,10 +499,10 @@ static int compute_accuracy_impl(const Table &t, int bitlevel, const char *quest
     CKE(bqeps.alloc(nq * sizeof(float)));
     CKE(bcnt.alloc(2 * sizeof(unsigned long long)));
     if (!simt) CKE(bcand.alloc(cand_cap * sizeof(tc::Candidate)));
-    float *dM = bM.as<float>(), *dQ = bQ.as<float>();
+    float *dM = nullptr, *dQ = bQ.as<float>();
     int *dq3 = bq3.as<int>();
     unsigned long long *dbest = bbest.as<unsigned long long>(), *dcnt = bcnt.as<unsigned long long>();
-    if ((rc = upload_fp32(t, dM, Dp))) return rc;
+    if ((rc = upload_fp32(t, bM, Dp, &dM))) return rc;
     CKE(cudaMemset(dQ, 0, (size_t)nq * Dp * sizeof(float)));
     CKE(cudaMemcpy(dq3, q3.data(), q3.size() * sizeof(int), cudaMemcpyHostToDevice));
     CKE(cudaMemset(dbest, 0, nq * sizeof(unsigned long long)));
@@ -1177,17 +1226,6 @@ template <int BITS> int topk_packed(BitsState &st, bool simt, TopkBufs &b, w2b_t
   return W2B_OK;
 }
 
-// bit level of a packed file (three integers on its first line, as accuracy_main.cpp tells them apart), else 0
-int packed_bits_of(const char *path) {
-  long long words, size, bits = 0;
-  char line[128], extra;
-  if (FILE *f = fopen(path, "rb")) {
-    if (!fgets(line, sizeof line, f) || sscanf(line, "%lld %lld %lld %c", &words, &size, &bits, &extra) != 3) bits = 0;
-    fclose(f);
-  }
-  return (int)bits;
-}
-
 // t: the table (names only matter when cap_queries > 0: counting the queries needs no vectors); packed = t.bits, the
 // level of a packed file or of a context on the bit-domain route, 0 for an fp32 table.
 int topk_impl(const Table &t, int packed, int bitlevel, bool nearest, const char *input, int k, int device, int32_t *ids,
@@ -1236,16 +1274,16 @@ int topk_impl(const Table &t, int packed, int bitlevel, bool nearest, const char
     const bool simt = dbg && atoi(dbg) != 0;
     // fp32 table: uploaded and normalised once for every batch
     DevBuf bM;
+    float *dM = nullptr;
     const long long Dp = (size + tc::BK - 1) / tc::BK * tc::BK;
     if (!packed) {
       DevEvent e0, e1;
-      CKE(bM.alloc((size_t)words * Dp * sizeof(float)));
-      if ((rc = upload_fp32(t, bM.as<float>(), Dp))) return rc;
+      if ((rc = upload_fp32(t, bM, Dp, &dM))) return rc;
       CKE(cudaEventCreate(&e0.e));
       CKE(cudaEventCreate(&e1.e));
       CKE(cudaEventRecord(e0.e));
-      build_fp32(t, bM.as<float>(), Dp);
-      eval_normalize_kernel<<<(unsigned)((words + 7) / 8), 256>>>(bM.as<float>(), words, size, Dp, bitlevel);
+      build_fp32(t, dM, Dp);
+      eval_normalize_kernel<<<(unsigned)((words + 7) / 8), 256>>>(dM, words, size, Dp, bitlevel);
       CKE(cudaEventRecord(e1.e));
       CKE(cudaEventSynchronize(e1.e));
       CKE(cudaEventElapsedTime(&s.gpu_ms, e0.e, e1.e));
@@ -1259,7 +1297,7 @@ int topk_impl(const Table &t, int packed, int bitlevel, bool nearest, const char
       TopkBufs b;
       if ((rc = topk_alloc(b, nb, k))) return rc;
       if (!packed) {
-        rc = topk_fp32(bM.as<float>(), words, size, sub, simt, b, s, &s.gpu_ms);
+        rc = topk_fp32(dM, words, size, sub, simt, b, s, &s.gpu_ms);
       } else {
         BitsState st;
         st.ctx = t.ctx;
@@ -1292,15 +1330,18 @@ int topk_impl(const Table &t, int packed, int bitlevel, bool nearest, const char
 
 int topk_file(const char *vectors_file, int bitlevel, int64_t threshold, bool nearest, const char *input, int k,
               int device, int32_t *ids, float *scores, int64_t cap_queries, int64_t *n_queries, w2b_topk_stats *stats) {
-  const int packed = packed_bits_of(vectors_file);
+  int bits;
+  const int kind = vector_kind(vectors_file, &bits);
+  const int packed = kind == W2B_VECTORS_PACKED ? bits : 0;
   if (packed && bitlevel != 0 && bitlevel != packed) {
     w2b_set_error("%s holds %d-bit vectors: bitlevel must be %d or 0", vectors_file, packed, packed);
     return W2B_EINVAL;
   }
   Table t;
   if (cap_queries > 0) {  // (counting the queries needs no vectors: no word is then in the vocabulary)
-    const int rc = packed ? read_packed(vectors_file, threshold, t.names, t.rows, t.words, t.size, t.bits)
-                          : read_vectors(vectors_file, threshold, t.names, t.M, t.words, t.size);
+    const int rc = packed                        ? read_packed(vectors_file, threshold, t.names, t.rows, t.words, t.size, t.bits)
+                   : kind == W2B_VECTORS_TEXT ? read_text(vectors_file, threshold, device, t)
+                                              : read_vectors(vectors_file, threshold, t.names, t.M, t.words, t.size);
     if (rc) return rc;
   }
   return topk_impl(t, packed, bitlevel, nearest, input, k, device, ids, scores, cap_queries, n_queries, stats);

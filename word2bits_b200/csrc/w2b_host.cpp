@@ -3,6 +3,7 @@
 // host glue (src/word2bits.cpp:112-301, :560-576, :614-618) with identical results;
 // the text is read once through mmap and tokenised into an int32 id stream instead of
 // being re-parsed with fgetc by every thread in every epoch (:396).
+#include <ctype.h>
 #include <fcntl.h>
 #include <math.h>
 #include <stdio.h>
@@ -15,6 +16,7 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
+#include <memory>
 #include <functional>
 #include <numeric>
 #include <string>
@@ -23,6 +25,7 @@
 
 #include "w2b.h"
 #include "w2b_internal.h"
+#include "w2b_text.cuh"
 
 void w2b_unigram_bounds(const int64_t *cn, int64_t V, int32_t *start) {
   const double N = (double)W2B_TABLE_SIZE;
@@ -867,6 +870,188 @@ static int w2b_read_packed_impl(const char *path, float *vec, char *words, int m
       const int64_t bit = j * bits;
       vec[a * D + j] = level_value((row[bit >> 3] >> (bit & 7)) & ((1 << bits) - 1), bits);
     }
+  }
+  return W2B_OK;
+}
+
+// ------------------------------------------------------------------------- text vector files (-binary 0)
+extern "C" int w2b_host_parse_floats(const char *text, int64_t n_bytes, float *out, int64_t cap, int64_t *n) {
+  if ((!text && n_bytes > 0) || n_bytes < 0 || (!out && cap > 0) || cap < 0 || !n) {
+    w2b_set_error("w2b_host_parse_floats: bad argument");
+    return W2B_EINVAL;
+  }
+  const char *p = text, *end = text + n_bytes;
+  int64_t k = 0;
+  for (;;) {
+    while (p < end && w2b::text::is_space(*p)) ++p;
+    if (p == end) break;
+    const char *e = w2b::text::token_end(p, end);
+    if (k >= cap) {
+      w2b_set_error("w2b_host_parse_floats: more than %lld tokens", (long long)cap);
+      return W2B_EINVAL;
+    }
+    if (!w2b::text::parse_token(p, e, out + k)) {
+      w2b_set_error("token %lld '%.*s' is not a number", (long long)k, (int)std::min<long long>(e - p, 64), p);
+      *n = k;
+      return W2B_EIO;
+    }
+    ++k;
+    p = e;
+  }
+  *n = k;
+  return W2B_OK;
+}
+
+namespace {
+// A FILE read through a large buffer, for walking the rows of a vector file.
+struct ByteReader {
+  FILE *f;
+  std::vector<char> buf = std::vector<char>(1 << 20);
+  size_t pos = 0, len = 0;
+  bool fill() {
+    pos = 0;
+    len = fread(buf.data(), 1, buf.size(), f);
+    return len > 0;
+  }
+  int get() { return (pos < len || fill()) ? (unsigned char)buf[pos++] : EOF; }
+  // past the next '\n' (or to the end); the bytes before it are appended to *line when line is set
+  void line_rest(std::string *line) {
+    for (;;) {
+      if (pos == len && !fill()) return;
+      const char *s = buf.data() + pos, *nl = (const char *)memchr(s, '\n', len - pos);
+      const size_t k = nl ? (size_t)(nl - s) : len - pos;
+      if (line) line->append(s, k);
+      pos += k + (nl ? 1 : 0);
+      if (nl) return;
+    }
+  }
+  void skip(int64_t k) {
+    for (; k > 0;) {
+      if (pos == len && !fill()) return;
+      const size_t t = (size_t)std::min<int64_t>(k, (int64_t)(len - pos));
+      pos += t;
+      k -= t;
+    }
+  }
+  // a name as read_vectors reads it: up to the first ' ' (not kept), '\n' skipped.  false at the end of the file.
+  bool name(std::string &w) {
+    w.clear();
+    int ch = get();
+    if (ch == EOF) return false;
+    for (; ch != EOF && ch != ' '; ch = get())
+      if (ch != '\n') w.push_back((char)ch);
+    return true;
+  }
+};
+
+// the header "V D" as fscanf reads it (read_vectors); the file is left right after D
+bool header2(FILE *f, long long &V, long long &D) { return fscanf(f, "%lld", &V) == 1 && fscanf(f, "%lld", &D) == 1; }
+}  // namespace
+
+// The one decision on a vector file's format (w2b.h w2b_vector_file_info).
+extern "C" int w2b_vector_file_info(const char *path, int64_t threshold, int *kind, int64_t *V, int64_t *D, int *bits) {
+  if (!path || !kind || !V || !D || !bits) { w2b_set_error("w2b_vector_file_info: null argument"); return W2B_EINVAL; }
+  return w2b_guarded("w2b_vector_file_info", [&]() -> int {
+    FILE *f = fopen(path, "rb");
+    if (!f) {
+      w2b_set_error("Input file not found");
+      return W2B_EIO;
+    }
+    std::unique_ptr<FILE, int (*)(FILE *)> closer(f, fclose);
+    *kind = W2B_VECTORS_BINARY;
+    *V = *D = 0;
+    *bits = 0;
+    char line[128], extra;
+    long long v = 0, d = 0, b = 0;
+    if (fgets(line, sizeof line, f) && sscanf(line, "%lld %lld %lld %c", &v, &d, &b, &extra) == 3) {
+      *kind = W2B_VECTORS_PACKED;  // three integers on the first line
+      *bits = (int)b;
+    } else {
+      rewind(f);
+      if (!header2(f, v, d)) return W2B_OK;  // read_vectors reports the bad header
+      if (d >= 1 && d <= (1LL << 20)) {
+        // (a) a binary row has '\n' right after its 4 D value bytes; (b) a text row is D tokens up to its '\n'
+        int ch;
+        while ((ch = fgetc(f)) != EOF && ch != ' ') {}
+        const long long sp = ftell(f) - 1;
+        if (ch == ' ' && sp >= 0 && fseek(f, sp + 1 + 4 * d, SEEK_SET) == 0 && fgetc(f) != '\n' &&
+            fseek(f, sp + 1, SEEK_SET) == 0) {
+          ByteReader r{f};
+          std::string row;
+          r.line_rest(&row);
+          const char *p = row.data(), *end = p + row.size();
+          long long tokens = 0;
+          bool ok = true;
+          for (;;) {
+            while (p < end && w2b::text::is_space(*p)) ++p;
+            if (p == end) break;
+            const char *e = w2b::text::token_end(p, end);
+            float x;
+            ok = ok && w2b::text::parse_token(p, e, &x) && ++tokens <= d;
+            if (!ok) break;
+            p = e;
+          }
+          if (ok && tokens == d) *kind = W2B_VECTORS_TEXT;
+        }
+      }
+    }
+    *V = (threshold > 0 && v > threshold) ? threshold : v;
+    *D = d;
+    return W2B_OK;
+  });
+}
+
+// The names of a vector file's rows, each as the evaluator compares it (w2b.h w2b_vector_names).
+extern "C" int w2b_vector_names(const char *path, int64_t threshold, char *names, int max_word, int64_t *n) {
+  if (!path || !names || max_word < 1 || !n) { w2b_set_error("w2b_vector_names: bad argument"); return W2B_EINVAL; }
+  return w2b_guarded("w2b_vector_names", [&]() -> int {
+    int kind, bits;
+    int64_t V, D;
+    int rc = w2b_vector_file_info(path, threshold, &kind, &V, &D, &bits);
+    if (rc) return rc;
+    FILE *f = fopen(path, "rb");
+    if (!f) {
+      w2b_set_error("Input file not found");
+      return W2B_EIO;
+    }
+    std::unique_ptr<FILE, int (*)(FILE *)> closer(f, fclose);
+    long long v, d;
+    char line[128];
+    if (kind == W2B_VECTORS_PACKED ? !fgets(line, sizeof line, f) : !header2(f, v, d)) {
+      w2b_set_error("bad header");
+      return W2B_EIO;
+    }
+    const int64_t row = kind == W2B_VECTORS_PACKED ? (D * bits + 7) / 8 + 1 : 4 * D;  // a packed row ends with '\n'
+    ByteReader r{f};
+    std::string w;
+    int64_t k = 0;
+    for (; k < V && r.name(w); ++k) {
+      char *out = names + k * max_word;
+      int j = 0;
+      for (; j < (int)w.size() && j < 50 && j < max_word - 1; ++j) out[j] = (char)toupper((unsigned char)w[j]);
+      out[j] = 0;
+      if (kind == W2B_VECTORS_TEXT)
+        r.line_rest(nullptr);
+      else
+        r.skip(row);
+    }
+    *n = k;
+    return W2B_OK;
+  });
+}
+
+// Row `row` of a text vector file: its name and the bytes of its values (w2b_internal.h).
+int w2b_text_row(const char *path, int64_t row, std::string &name, std::string &values) {
+  FILE *f = fopen(path, "rb");
+  if (!f) return W2B_EIO;
+  std::unique_ptr<FILE, int (*)(FILE *)> closer(f, fclose);
+  long long v, d;
+  if (!header2(f, v, d)) return W2B_EIO;
+  ByteReader r{f};
+  for (int64_t k = 0; k <= row; ++k) {
+    if (!r.name(name)) return W2B_EIO;
+    values.clear();
+    r.line_rest(k == row ? &values : nullptr);
   }
   return W2B_OK;
 }

@@ -5,6 +5,8 @@
 
 #include <exception>
 #include <new>
+#include <string>
+#include <vector>
 
 void w2b_set_error(const char *fmt, ...);
 
@@ -66,3 +68,10 @@ void w2b_keep_thresholds(const int64_t *cn, int64_t V, int64_t train_words, floa
 void w2b_gather_slices(const int32_t *ids, long long n_tokens, long long L, int nshards, const long long *cursor,
                        const int *done, int32_t *stage, long long *xlate, long long *limit, int *limit_is_eof,
                        int nthreads);
+// Text vector files (-binary 0, w2b_write_vectors(binary = 0)).  w2b_text_parse streams the first V rows of the file,
+// whose first row holds D values (w2b_vector_file_info said W2B_VECTORS_TEXT), into the device table M (zeroed by the
+// caller, rows Dp floats apart) on the current device, and returns each row's name as written ('\n' skipped).
+// W2B_EIO names the row and token of a malformed file.  W2B_TEXT_CHUNK_BYTES (test hook) sets the chunk size.
+int w2b_text_parse(const char *path, int64_t V, int64_t D, float *M, int64_t Dp, std::vector<std::string> &names);
+// Row `row` of a text vector file, read on the host: its name and the bytes of its values (for error messages).
+int w2b_text_row(const char *path, int64_t row, std::string &name, std::string &values);
